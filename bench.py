@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the Panacea denoising hot path on B200 (BASELINE.json metric: UNet denoise-steps/s).
+"""Benchmark of the Panacea denoising hot path on H100 (BASELINE.json metric: UNet denoise-steps/s).
 
 A "step" = one Euler/DDIM step of one 6-view x 8-frame sequence: CFG-doubled eps evaluation (ControlNet + UNet on
 16 frames of [8, 32, 6x56]) + guidance + update — BASELINE.json configs[1] ("single-GPU 50-step DDIM, 6 views x 8
@@ -48,7 +48,7 @@ def workload_config(n_gpus: int) -> dict:
                         "full-size UNet+ControlNet (2.24 B params, random init, zero-init tails re-drawn N(0,0.02^2))",
             "cfg_scale": 5.0, "frames": T, "views": VIEWS, "latent_hw_per_view": [H, W_VIEW],
             "sequences_per_gpu": 1, "parallelism": f"dp{n_gpus} (independent sequences, NCCL gather of final latents)",
-            "l2_policy": "no explicit flush: every step streams 4.5 GB of bf16 weights + >2 GB of activations, >> 126 MB L2"}
+            "l2_policy": "no explicit flush: every step streams 4.5 GB of bf16 weights + >2 GB of activations, >> 50 MB L2"}
 
 
 # ------------------------------------------------------------------------------------------------ clocks
@@ -220,7 +220,7 @@ def load_traffic():
 
 
 def profile_dominant_kernel(pipe, x_in, t_dev, cc):
-    """One eager eps-eval with CUDA-event timing around every launch of the dominant kernel (the tcgen05 GEMM /
+    """One eager eps-eval with CUDA-event timing around every launch of the dominant kernel (the wgmma GEMM /
     implicit-conv kernel): achieved TFLOP/s = sum of algorithmic FLOPs / sum of launch durations."""
     eng = pipe.model.engine()
     ops = eng.ops
@@ -260,6 +260,17 @@ def profile_dominant_kernel(pipe, x_in, t_dev, cc):
     return flops, secs, len(recs), sum(r[3] for r in recs)
 
 
+def dump_outputs(out_dir, arrays) -> None:
+    """What the last timed step computed, as float32 .npy files: eps (the CFG-doubled network output), latent (the
+    sample after the Euler update) and network_input (the scaled, duplicated latent of the next step); a few MB in all."""
+    import numpy as np
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(d / f"{name}.npy", t.detach().float().cpu().numpy())
+    log(f"outputs of the last timed step written to {d}")
+
+
 def run_ours(args) -> None:
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -273,6 +284,7 @@ def run_ours(args) -> None:
     from panacea_b200 import dist_utils as D
     seed = D.rank_seed(rank)                                       # inference.py:250: 3407 + rank
     log("building full-size UNet + ControlNet on the device")
+    torch.manual_seed(seed)                                        # same arguments -> same weights and inputs
     pipe = build_pipeline(dev, seed)
     log("synthetic host inputs (pinned)")
     host = synth_inputs_host(seed)
@@ -300,6 +312,7 @@ def run_ours(args) -> None:
         j = i % (len(sig) - 1)
         eps = wrapper(x_in, t_all[j], cc, return_static=True)
         ops.cfg_euler_step(x, eps, x_in, sig[j], sig[j + 1], 5.0, scal[j + 1][2] if j + 1 < len(scal) else scal[0][2], sigma_q=scal[j][1])
+        return eps
 
     for i in range(max(Wm, 3)):                                    # >= 3 warm-ups: packing, graph capture, clocks
         step(i)
@@ -321,13 +334,15 @@ def run_ours(args) -> None:
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record()
     for i in range(K):
-        step(i)
+        eps = step(i)
     ev1.record()
     torch.cuda.synchronize()
     if dist is not None:
         dist.barrier()
     ms = ev0.elapsed_time(ev1)
     log(f"timed region: {K} steps in {ms:.1f} ms")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"eps": eps, "latent": x, "network_input": x_in})
     clk = clocks.stop() if rank == 0 else None
     ms = D.max_over_ranks(ms, dev)
 
@@ -388,7 +403,7 @@ def run_ours(args) -> None:
             peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
         except (OSError, ValueError):
             pass
-        peak = peaks.get("bf16_tflops_sustained", 1400.0)
+        peak = peaks.get("bf16_tflops_sustained", 989.0)
         achieved = flops / secs / 1e12
         traffic, traffic_src = load_traffic()
         value = world * K / (ms * 1e-3)
@@ -403,12 +418,12 @@ def run_ours(args) -> None:
             "launches_per_step": launches_per_eps + 1,
             "algorithmic_tflop_per_step": ALGO_TFLOP_PER_STEP,
             "achieved_tflops_whole_step": ALGO_TFLOP_PER_STEP * (K / (ms * 1e-3)),
-            "roofline": {"bound": "tensor", "kernel": "pn::gemm_tc_kernel (tcgen05 GEMM / implicit conv, all launches of one eps-eval)",
+            "roofline": {"bound": "tensor", "kernel": "pn::gemm_tc_kernel (wgmma GEMM / implicit conv, all launches of one eps-eval)",
                          "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic,
                          "traffic_unit": "bytes per launch (DRAM read + write)", "traffic_source": traffic_src,
                          "algorithmic_bytes_per_launch": algo_bytes / max(n_gemm, 1),
                          "algorithmic_flops_per_launch": flops / max(n_gemm, 1),
-                         "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "fallback 1400",
+                         "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "H100 SXM data sheet, dense BF16 (989)",
                          "launches": n_gemm, "share_of_step": secs / (ms * 1e-3 / K),
                          "how": "sum of 2*M*N*K over the launches / sum of per-launch CUDA-event durations, eager pass after the timed region"},
             "clocks": clk, "cpu_baseline": cpu,
@@ -425,6 +440,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)
@@ -436,7 +453,8 @@ def main():
         # convenience: self-launch under torchrun when started as a plain script
         cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={args.gpus}", "--master-addr", "127.0.0.1",
                "--master-port", os.environ.get("MASTER_PORT", "29511"), str(Path(__file__).resolve()), "--gpus", str(args.gpus), "--steps",
-               str(args.steps), "--warmup", str(args.warmup)] + (["--no-cpu-baseline"] if args.no_cpu_baseline else [])
+               str(args.steps), "--warmup", str(args.warmup)] + (["--no-cpu-baseline"] if args.no_cpu_baseline else []) + \
+              (["--dump-outputs", args.dump_outputs] if args.dump_outputs else [])
         raise SystemExit(subprocess.call(cmd))
     run_ours(args)
 

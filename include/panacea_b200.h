@@ -1,5 +1,5 @@
 /*
- * panacea_b200 — C ABI of the B200-native Panacea denoising hot path.
+ * panacea_b200 — C ABI of the H100-native Panacea denoising hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b). The reference is pure Python with no FFI of its own; the
  * interface this library stands behind is the `nn.Module.forward` surface of
@@ -46,7 +46,7 @@ const char* pn_last_error(void);
 int pn_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------------
- * pn_gemm — tcgen05 GEMM / implicit-GEMM convolution (sm_100a, TMA + TMEM).
+ * pn_gemm — wgmma GEMM / implicit-GEMM convolution (sm_90a, TMA + mbarrier pipeline).
  * Replaces: nn.Linear (attention.py:94,113,220-226; openaimodel.py:939-941), nn.Conv2d 3x3 stride 1 over
  * the 6-view panorama (openaimodel.py:413,455-462,125), nn.Conv1d k=3 over frames (openaimodel.py:418,
  * 468-476), 1x1 skip / zero convs (openaimodel.py:486; controlmodel.py:81-84).
@@ -74,9 +74,9 @@ typedef struct pn_gemm_args {
   int32_t geglu;
   int32_t residual_bf16;  /* the residual is bf16 (bf16 output only): the transformer blocks' bf16 token stream */
   /* LayerNorm folded into the GEMMs around the bf16 token stream (attention.py:699-701 + :726-747, norm1/2/3):
-   * ln_stats_out — this GEMM (1x1, K <= 640, bf16 out) also writes, per output row, pn_gemm_ln_parts(N) partial
+   * ln_stats_out — this GEMM (bf16 out, no GEGLU) also writes, per output row, pn_gemm_ln_parts(N) partial
    *   (sum, sum of squares) pairs of the bf16 values it stores: float [rows][parts][2];
-   * ln_stats_in / ln_parts_in / ln_colsum / ln_eps — (1x1, K <= 640, bf16 out, no GEGLU) A is the UN-normalised stream, B = W diag(gamma); the epilogue
+   * ln_stats_in / ln_parts_in / ln_colsum / ln_eps — (1x1, bf16 out, no GEGLU) A is the UN-normalised stream, B = W diag(gamma); the epilogue
    *   finishes the LayerNorm: out = rstd_m (acc - mean_m s_n) + bias_n with s_n = ln_colsum[n] = sum_k B[n,k] and the
    *   caller's bias_n = sum_k beta_k W[n,k] (+ the layer's own bias); mean/rstd over the C = K channels of row m. */
   const float* ln_stats_in;
@@ -90,7 +90,7 @@ int pn_gemm(const pn_gemm_args* args, void* stream);
 int pn_gemm_ln_parts(int N);
 
 /* ------------------------------------------------------------------------------------------------
- * pn_attention — tcgen05 flash attention over view-tiled tokens (head_dim 64).
+ * pn_attention — wgmma flash attention over view-tiled tokens (head_dim 64).
  * Replaces: xformers.ops.memory_efficient_attention inside MemoryEfficientIntraViewAttention.forward
  * (attention.py:407-489) and MemoryEfficientInterViewAttentionTwo.forward (attention.py:518-610), and
  * F.scaled_dot_product_attention inside CrossAttention.forward for the 77-token text context

@@ -8,6 +8,7 @@ from seeds by whoever consumes a fixture.
 from __future__ import annotations
 
 import argparse
+import hashlib
 import sys
 import time
 from pathlib import Path
@@ -173,6 +174,33 @@ def sampler_inputs(case: Cs.EpsCase, use_last_frame: bool = False):
     return x, c, uc
 
 
+def state_spec_digest(spec: dict) -> str:
+    """sha256 of the sorted 'key shape' lines of a state-dict spec (2,478 keys: the digest keeps the fixture small)."""
+    lines = "\n".join(f"{k} {tuple(int(d) for d in v)}" for k, v in sorted(spec.items()))
+    return hashlib.sha256(lines.encode()).hexdigest()
+
+
+@torch.no_grad()
+def golden_reference_model() -> dict:
+    """What tests/test_oracle_vs_reference.py compares the port with: the reference model's state-dict shapes and its
+    output on GOLDEN_CASES[1] (non-2:1 views: exercises the view-height shim), and a FRESH reference model's output on
+    GOLDEN_CASES[0] (zero_module'd tails: exactly 0)."""
+    case = Cs.GOLDEN_CASES[1]
+    model = R.build_reference_model(case.unet_kwargs())
+    spec = {k: tuple(v.shape) for k, v in model.state_dict().items()}
+    model.load_state_dict(Cs.make_weights(case), strict=True)
+    x, t, c = Cs.make_inputs(case)
+    with R.view_height_shim(case.H, case.w):
+        eps = model(x, t, dict(c))
+    case0 = Cs.GOLDEN_CASES[0]
+    fresh = R.build_reference_model(case0.unet_kwargs())
+    x0, t0, c0 = Cs.make_inputs(case0)
+    eps_fresh = fresh(x0, t0, dict(c0))
+    return {"case": case.name, "state_spec_sha256": state_spec_digest(spec), "state_spec_len": len(spec),
+            "eps": eps.contiguous(), "fresh_case": case0.name, "fresh_max_abs": eps_fresh.abs().max().item(),
+            "torch": str(torch.__version__)}
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--only", default="")
@@ -180,6 +208,9 @@ def main(argv=None):
     a = ap.parse_args(argv)
     only = set(filter(None, a.only.split(",")))
     GOLDEN.mkdir(parents=True, exist_ok=True)
+    if not only or "reference_model" in only:
+        torch.save(golden_reference_model(), GOLDEN / "reference_model.pt")
+        print("reference_model.pt")
     if not only or "kat" in only:
         torch.save(golden_kat(), GOLDEN / "kat.pt")
         print("kat.pt")

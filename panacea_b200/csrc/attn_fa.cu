@@ -1,4 +1,4 @@
-// tcgen05 flash attention for the decomposed-4D attention of Panacea (head_dim 64 — the reference config — or 80,
+// wgmma flash attention for the decomposed-4D attention of Panacea (head_dim 64 — the reference config — or 80,
 // BASELINE.json configs[4]; bf16 operands, fp32 softmax).
 //
 // One kernel serves the three tensor-core attention variants; they differ only in which K/V tiles a query tile
@@ -10,48 +10,38 @@
 //   * text cross-attention (attention.py:229-291, 77 keys): V=1, one K/V block per batch element, tail masked.
 // (Temporal self-attention over T<=16 frames is a CUDA-core kernel, attn_small.cu.)
 //
-// CTA = a PAIR of query tiles (<=128 queries each, consecutive tiles of one frame/view/head) that share the K/V
-// stream, one softmax warpgroup per tile so the two tiles' dependency chains interleave on the tensor core and the
-// MUFU. Warp roles:
-//   warp 0: TMA producer (Q pair, double buffered across work items; K and V boxes through a 4-stage ring)
-//   warp 1: UMMA issuer   S_t = Q_t K^T  (M=128, N=kv_n, K=64)  SS form -> TMEM
-//                         O_t (+)= P_t V (M=128, N=64,  K=kv_n) TS form: P is read from TENSOR MEMORY, V is the
-//                                                               MN-major B operand; O accumulates in TMEM
-//   warps 2-5 / 6-9: softmax group of tile A / B, ONE thread per query row (TMEM lane == row): tcgen05.ld S ->
-//              row max -> exp2 -> bf16 P written back to TMEM (tcgen05.st); the running maximum is only raised when
-//              it grew by more than 2^8 (lazy rescale, exact: l and O always share one reference maximum), and the
-//              rare rescale of O is done in place in TMEM by the row's own thread. The normalise-and-store epilogue
-//              of a work item runs inside the first block of the next one, behind that block's S MMA.
+// CTA = one query tile (<= 128 queries of one frame/view/head), 288 threads:
+//   warps 0-3 / 4-7: two consumer warpgroups, query rows 0-63 / 64-127. Per key block of <= 128 keys:
+//                    S = Q K^T   wgmma m64n128k16, Q and K K-major from shared memory (fp32 S in registers);
+//                    online softmax in registers (a query row lives in the 4 lanes of a quad);
+//                    O += P V    wgmma m64n64k16 with P as the REGISTER A operand (the S accumulator fragment is the
+//                                A fragment layout) and V the MN-major B operand from shared memory.
+//   warp 8:          TMA producer (Q once, K and V boxes through a STAGES-deep mbarrier ring).
+// head_dim 80 is a 64-channel part plus a 16-channel part (a TMA box with a 128 B swizzle cannot be wider than 64
+// bf16): every Q/K/V tile has a second, 32 B-row tile; S gets a fifth K = 16 step on the 16-channel tiles and
+// O = P V a second wgmma of N = 16 per key step into output channels 64..79.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/panacea_b200.h"
 
 namespace pn {
 
-constexpr int FA_THREADS = 320;   // warp 0 TMA, warp 1 MMA, warps 2..5 softmax of tile A, 6..9 of tile B
+constexpr int FA_THREADS = 288;
 constexpr int FA_TILE_BYTES = 128 * 128;          // 128 rows x 64 bf16 (128 B rows, 128B swizzle)
 constexpr int FA_XTILE_BYTES = 128 * 32;          // head_dim 80: the channels 64..79 of 128 rows (32 B rows, 32B swizzle)
-// Shared / tensor memory layout per head_dim. head_dim 80 is handled as a 64-channel part plus a 16-channel part (a
-// TMA box with a 128 B swizzle cannot be wider than 64 bf16): every Q/K/V tile has a second, 32 B-row tile; S gets a
-// fifth K = 16 MMA step on the 16-channel tiles and O = P V a second MMA of N = 16 per key step into O columns 64..79.
+constexpr int FA_MAX_KEYS = 128;                  // keys per block = the N of the S wgmma
+
 template <int D>
 struct FaL {
-  static constexpr int STAGES = D == 64 ? 4 : 3;                     // K/V ring (227 KB of shared memory)
+  static constexpr int STAGES = 3;
   static constexpr int XB = D == 64 ? 0 : FA_XTILE_BYTES;
-  static constexpr int Q = 0;                                        // [2 buffers][2 tiles]
-  static constexpr int K = 4 * FA_TILE_BYTES;
-  static constexpr int V = K + STAGES * FA_TILE_BYTES;
-  static constexpr int QX = V + STAGES * FA_TILE_BYTES;
-  static constexpr int KX = QX + 4 * XB;
-  static constexpr int VX = KX + STAGES * XB;
-  static constexpr int BAR = VX + STAGES * XB;
-  static constexpr int TOTAL = BAR + 512 + 1024;
-  // tensor memory columns. d = 64: S_A S_B (fp32, 128 each) | P_A P_B (bf16 pairs, 64 each) | O_A O_B (fp32, 64 each);
-  // d = 80 (key blocks of <= 112 keys): S 2 x 112 | P 2 x 56 | O 2 x 80 = 496 columns.
-  static constexpr uint32_t S_STRIDE = D == 64 ? 128 : 112, P_BASE = D == 64 ? 256 : 224, P_STRIDE = D == 64 ? 64 : 56;
-  static constexpr uint32_t O_BASE = D == 64 ? 384 : 336, O_STRIDE = D;
+  static constexpr int Q = 0;
+  static constexpr int QX = FA_TILE_BYTES;
+  static constexpr int KV = FA_TILE_BYTES + XB;                 // stage s: [K | V | Kx | Vx]
+  static constexpr int STAGE_BYTES = 2 * FA_TILE_BYTES + 2 * XB;
+  static constexpr int BAR = KV + STAGES * STAGE_BYTES;
+  static constexpr int TOTAL = BAR + 128 + 1024;
 };
-constexpr float FA_LAZY_LOG2 = 8.0f;              // raise the reference maximum only when it grew by more than 2^8
 
 struct FaParams {
   CUtensorMap mapQ;
@@ -61,448 +51,202 @@ struct FaParams {
   int heads;
   int F, H, V, W;              // query token grid
   int qw, qh, tiles_x, tiles_y;
-  int tiles_per_group, pairs;  // query tiles of one (frame, view, head) and pairs of them
-  int kw, kh, kv_rows, kv_n, kv_yblocks;
+  int tiles_per_group;         // query tiles of one (frame, view, head)
+  int kw, kh, kv_rows, kv_yblocks;
   int kv_views[8][2];
   int kv_view_count[8];
   int kv_frame_div;            // kv frame = q frame / kv_frame_div
-  int total_items;
   float scale_log2;            // softmax scale * log2(e)
-#ifdef PN_GEMM_ROLE_TIMERS
-  int debug;                   // diagnostics builds only — PN_ATTN_DEBUG: 1 = no softmax math, 2 = no MMA issue, 4 = no rendezvous
-#endif
   __nv_bfloat16* out;
   long long out_ld;            // token stride of out (elements)
 };
 
-// Timeline of CTA 0 (diagnostics builds, PN_ATTN_DEBUG=8): clock64 stamps of the two softmax groups and of the UMMA issuer
-// per key block — tools/attn_timeline.py prints the phase durations.
-//  group g (0|1), block n: [g][n][0] S ready  [1] S in registers  [2] row maximum done  [3] past the rendezvous
-//  [4] exponentials done  [5] previous PV retired  [6] P stored;   issuer: [2][n][0|1] S issued (slot A|B), [2|3] PV issued
-#ifdef PN_GEMM_ROLE_TIMERS
-constexpr int FA_TL_BLOCKS = 96;
-__device__ long long g_fa_tl[3][FA_TL_BLOCKS][8];
-#define FA_STAMP(cond, g, n, e) do { if ((cond) && (n) < (uint32_t)FA_TL_BLOCKS) g_fa_tl[g][n][e] = clock64(); } while (0)
-#else
-#define FA_STAMP(cond, g, n, e) do { } while (0)
-#endif
-
-struct FaItem {
-  int t0, head, view, frame, nblk;
-  bool has_b;
-};
-
-// pair fastest, then head, view, frame: CTAs that run concurrently share K/V in L2
-__device__ __forceinline__ FaItem fa_decode(const FaParams& p, int item) {
-  FaItem t;
-  const int pr = item % p.pairs; item /= p.pairs;
-  t.head = item % p.heads; item /= p.heads;
-  t.view = item % p.V; item /= p.V;
-  t.frame = item;
-  t.t0 = 2 * pr;
-  t.has_b = (t.t0 + 1) < p.tiles_per_group;
-  t.nblk = p.kv_view_count[t.view] * p.kv_yblocks;
-  return t;
-}
-
-// Persistent kernel: each CTA walks a strided list of work items; the K/V-block pipeline runs ACROSS item boundaries
-// (Q double buffer, deferred epilogue), which is what lets the 1-block text attention and the 16/32-block view attention
-// share one kernel.
-// MASK: the key block has padding columns (kv_rows < kv_n, e.g. 77 text keys in an 80-wide block) that must get p = 0.
-// NCH: number of 16-column chunks of a key block (kv_n / 16) fixed at compile time for the shapes of the network
-// (7 = 112 keys per block at 32x56 views, 8 = 128 keys at 32x64 views, 5 = the 77 text keys, 2 = the 4x7 middle block);
-// 0 = read it from the parameters (any other shape).
-template <bool MASK, int NCH, int D>
+template <int D>
 __global__ void __launch_bounds__(FA_THREADS, 1) attn_fa_kernel(const __grid_constant__ FaParams p) {
   using L = FaL<D>;
-  constexpr int FA_STAGES = L::STAGES;
-  constexpr int FA_D = D;
+  constexpr int STAGES = L::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::BAR);
-  uint64_t* q_full = bars;                     // [2]
-  uint64_t* q_empty = bars + 2;                // [2]
-  uint64_t* k_full = bars + 4;                 // [FA_STAGES]
-  uint64_t* v_full = bars + 8;                 // [FA_STAGES]
-  uint64_t* kv_empty = bars + 12;              // [FA_STAGES]
-  uint64_t* s_full = bars + 16;                // [2 tiles]  S_t written by the tensor core
-  uint64_t* s_free = bars + 18;                // [2]        S_t copied to registers by its softmax group
-  uint64_t* p_full = bars + 20;                // [2]        P_t (and a rescaled O_t) complete in tensor memory
-  uint64_t* pv_done = bars + 22;               // [2]        O_t (+)= P_t V retired: P_t and O_t may be touched again
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 24);
+  uint64_t* q_full = bars;                     // [1]
+  uint64_t* kv_full = bars + 1;                // [STAGES]
+  uint64_t* kv_empty = bars + 1 + STAGES;      // [STAGES]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-#ifdef PN_GEMM_ROLE_TIMERS
-  const int dbgmode = p.debug;
-#else
-  constexpr int dbgmode = 0;
-#endif
 
-  // zero Q/K/V staging once: rows a TMA box does not cover (kv_rows..kv_n) must read as 0, never as stale NaNs
+  // zero Q/K/V staging once: rows a TMA box does not cover (keys kv_rows..127, queries beyond the tile) must read as 0,
+  // never as stale NaNs
   {
     uint4* z = reinterpret_cast<uint4*>(smem);
     for (int i = threadIdx.x; i < L::BAR / 16; i += FA_THREADS) z[i] = make_uint4(0, 0, 0, 0);
     fence_proxy_async_smem();
   }
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.mapQ);
-    tma_prefetch_desc(&p.mapK);
-    tma_prefetch_desc(&p.mapV);
-    if (D == 80) { tma_prefetch_desc(&p.mapQx); tma_prefetch_desc(&p.mapKx); tma_prefetch_desc(&p.mapVx); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&q_full[i], 1); mbar_init(&q_empty[i], 1); }
-    for (int i = 0; i < FA_STAGES; ++i) { mbar_init(&k_full[i], 1); mbar_init(&v_full[i], 1); mbar_init(&kv_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_free[i], 4);       // one elected arrive per warp of the tile's softmax group
-      mbar_init(&p_full[i], 4);
-      mbar_init(&pv_done[i], 1);
-    }
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_prologue_done();
 
-  if (warp == 0) {
+  // query tile fastest, then head, view, frame: CTAs that run concurrently share K/V in L2
+  int item = blockIdx.x;
+  const int ti = item % p.tiles_per_group; item /= p.tiles_per_group;
+  const int head = item % p.heads; item /= p.heads;
+  const int view = item % p.V;
+  const int frame = item / p.V;
+  const int nblk = p.kv_view_count[view] * p.kv_yblocks;
+
+  if (warp == 8) {
     // ===================== TMA producer (warp-wide loop, TMA issue under elect.sync) =====================
-    {
-      const uint32_t q_bytes = (uint32_t)(p.qw * p.qh) * (D == 80 ? 160u : 128u);
-      const uint32_t kv_bytes = (uint32_t)p.kv_rows * (D == 80 ? 160u : 128u);
-      int g = 0, it = 0;
-      for (int item = blockIdx.x; item < p.total_items; item += gridDim.x, ++it) {
-        const FaItem t = fa_decode(p, item);
-        const int qb = it & 1;
-        mbar_wait(&q_empty[qb], (uint32_t)(((it >> 1) & 1) ^ 1));
-        if (elect_one()) {
-          mbar_arrive_expect_tx(&q_full[qb], t.has_b ? 2 * q_bytes : q_bytes);
-          for (int sl = 0; sl < (t.has_b ? 2 : 1); ++sl) {
-            const int ti = t.t0 + sl;
-            tma_load_5d(smem + L::Q + (qb * 2 + sl) * FA_TILE_BYTES, &p.mapQ, &q_full[qb], t.head * FA_D,
-                        (ti % p.tiles_x) * p.qw, t.view, (ti / p.tiles_x) * p.qh, t.frame);
-            if (D == 80)
-              tma_load_5d(smem + L::QX + (qb * 2 + sl) * FA_XTILE_BYTES, &p.mapQx, &q_full[qb], t.head * FA_D + 64,
-                          (ti % p.tiles_x) * p.qw, t.view, (ti / p.tiles_x) * p.qh, t.frame);
-          }
-        }
-        const int kv_frame = t.frame / p.kv_frame_div;
-        int vi = 0, yb = 0;
-        for (int j = 0; j < t.nblk; ++j, ++g) {
-          const int st = g % FA_STAGES;
-          const int kvv = p.kv_views[t.view][vi];
-          mbar_wait(&kv_empty[st], (uint32_t)(((g / FA_STAGES) & 1) ^ 1));
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&k_full[st], kv_bytes);
-            tma_load_5d(smem + L::K + st * FA_TILE_BYTES, &p.mapK, &k_full[st], t.head * FA_D, 0, kvv, yb * p.kh, kv_frame);
-            if (D == 80) tma_load_5d(smem + L::KX + st * FA_XTILE_BYTES, &p.mapKx, &k_full[st], t.head * FA_D + 64, 0, kvv, yb * p.kh, kv_frame);
-            mbar_arrive_expect_tx(&v_full[st], kv_bytes);
-            tma_load_5d(smem + L::V + st * FA_TILE_BYTES, &p.mapV, &v_full[st], t.head * FA_D, 0, kvv, yb * p.kh, kv_frame);
-            if (D == 80) tma_load_5d(smem + L::VX + st * FA_XTILE_BYTES, &p.mapVx, &v_full[st], t.head * FA_D + 64, 0, kvv, yb * p.kh, kv_frame);
-          }
-          if (++yb == p.kv_yblocks) { yb = 0; ++vi; }
-        }
-      }
+    const uint32_t q_bytes = (uint32_t)(p.qw * p.qh) * (D == 80 ? 160u : 128u);
+    const uint32_t kv_bytes = (uint32_t)p.kv_rows * (D == 80 ? 160u : 128u);
+    if (elect_one()) {
+      tma_prefetch_desc(&p.mapQ);
+      tma_prefetch_desc(&p.mapK);
+      tma_prefetch_desc(&p.mapV);
+      mbar_arrive_expect_tx(q_full, q_bytes);
+      const int x0 = (ti % p.tiles_x) * p.qw, y0 = (ti / p.tiles_x) * p.qh;
+      tma_load_5d(smem + L::Q, &p.mapQ, q_full, head * D, x0, view, y0, frame);
+      if (D == 80) tma_load_5d(smem + L::QX, &p.mapQx, q_full, head * D + 64, x0, view, y0, frame);
     }
-  } else if (warp == 1) {
-    // ===================== UMMA issuer (warp-wide loop; MMAs and commits under elect.sync, descriptors = base + k) ====
-    {
-      const uint32_t idesc_s = umma_idesc_bf16(128, p.kv_n, 0, 0);      // S = Q K^T : both K-major
-      const uint32_t idesc_pv = umma_idesc_bf16(128, 64, 0, 1);         // PV: A = P (tensor memory), B = V MN-major
-      const uint32_t idesc_pvx = umma_idesc_bf16(128, 16, 0, 1);        // head_dim 80: channels 64..79
-      const int ksteps_pv = NCH > 0 ? NCH : p.kv_n / 16;
-      const uint64_t dQ0 = umma_smem_desc(smem_u32(smem + L::Q), 16, 1024);
-      const uint64_t dK0 = umma_smem_desc(smem_u32(smem + L::K), 16, 1024);
-      const uint64_t dV0 = umma_smem_desc(smem_u32(smem + L::V), 1024, 1024);
-      // 16-channel tiles: 32 B rows, 32B swizzle, 8-row groups 256 B apart (K-major for Q/K, MN-major for V)
-      const uint64_t dQx0 = umma_smem_desc_sw32(smem_u32(smem + L::QX), 16, 256);
-      const uint64_t dKx0 = umma_smem_desc_sw32(smem_u32(smem + L::KX), 16, 256);
-      const uint64_t dVx0 = umma_smem_desc_sw32(smem_u32(smem + L::VX), 256, 256);
-      constexpr uint64_t TILE_STEP = FA_TILE_BYTES >> 4;                // start-address field is in 16-byte units
-      constexpr uint64_t XTILE_STEP = FA_XTILE_BYTES >> 4;
-      uint32_t n_s[2] = {0, 0}, n_pv[2] = {0, 0};                       // blocks issued per tile slot
-      bool pend = false, pend_b = false;
-      int pend_g = 0, pend_j = 0;
-      // O_t (+)= P_t V of the block issued one iteration earlier (its softmax ran while the next S was computed)
-      auto issue_pv = [&]() {
-        const int st = pend_g % FA_STAGES;
-        mbar_wait(&v_full[st], (uint32_t)((pend_g / FA_STAGES) & 1));
-        const uint64_t dV = dV0 + TILE_STEP * st;
-#pragma unroll
-        for (int sl = 0; sl < 2; ++sl) {
-          if (sl == 0 || pend_b) {
-            mbar_wait(&p_full[sl], n_pv[sl] & 1);
-            tc_fence_after();
-            if (elect_one()) {
-              const uint32_t tO = tmem_base + L::O_BASE + sl * L::O_STRIDE, tP = tmem_base + L::P_BASE + sl * L::P_STRIDE;
-              const uint64_t dVx = dVx0 + XTILE_STEP * st;
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {  // 16 keys per step: 8 packed columns of P, 16 rows (128 B each) of V
-                if (k < ksteps_pv && dbgmode != 2) {
-                  umma_f16_ts(tO, tP + 8 * k, dV + 128 * k, idesc_pv, (pend_j > 0 || k > 0) ? 1u : 0u);
-                  if (D == 80) umma_f16_ts(tO + 64, tP + 8 * k, dVx + 32 * k, idesc_pvx, (pend_j > 0 || k > 0) ? 1u : 0u);
-                }
-              }
-              umma_commit(&pv_done[sl]);
-              FA_STAMP(dbgmode == 8 && blockIdx.x == 0, 2, n_pv[sl], 2 + sl);
-              if (sl == 1 || !pend_b) umma_commit(&kv_empty[st]);
-            }
-            ++n_pv[sl];
-          }
-        }
-      };
-      int g = 0, it = 0;
-      for (int item = blockIdx.x; item < p.total_items; item += gridDim.x, ++it) {
-        const FaItem t = fa_decode(p, item);
-        const int qb = it & 1;
-        mbar_wait(&q_full[qb], (uint32_t)((it >> 1) & 1));
-        for (int j = 0; j < t.nblk; ++j, ++g) {
-          const int st = g % FA_STAGES;
-          mbar_wait(&k_full[st], (uint32_t)((g / FA_STAGES) & 1));
-          const uint64_t dK = dK0 + TILE_STEP * st;
-#pragma unroll
-          for (int sl = 0; sl < 2; ++sl) {
-            if (sl == 0 || t.has_b) {
-              mbar_wait(&s_free[sl], (n_s[sl] & 1) ^ 1);
-              tc_fence_after();
-              if (elect_one()) {
-                const uint64_t dQ = dQ0 + TILE_STEP * (qb * 2 + sl);
-                if (dbgmode != 2) {
-#pragma unroll
-                  for (int k = 0; k < 4; ++k)
-                    umma_f16_ss(tmem_base + sl * L::S_STRIDE, dQ + 2 * k, dK + 2 * k, idesc_s, k > 0 ? 1u : 0u);
-                  if (D == 80)
-                    umma_f16_ss(tmem_base + sl * L::S_STRIDE, dQx0 + XTILE_STEP * (qb * 2 + sl), dKx0 + XTILE_STEP * st, idesc_s, 1u);
-                }
-                umma_commit(&s_full[sl]);
-                FA_STAMP(dbgmode == 8 && blockIdx.x == 0, 2, n_s[sl], sl);
-                // every S MMA reading this Q pair has retired
-                if (j == t.nblk - 1 && (sl == 1 || !t.has_b)) umma_commit(&q_empty[qb]);
-              }
-              ++n_s[sl];
-            }
-          }
-          if (pend) issue_pv();
-          pend = true; pend_b = t.has_b; pend_g = g; pend_j = j;
+    const int kv_frame = frame / p.kv_frame_div;
+    int vi = 0, yb = 0;
+    for (int j = 0; j < nblk; ++j) {
+      const int st = j % STAGES;
+      const int kvv = p.kv_views[view][vi];
+      mbar_wait(&kv_empty[st], (uint32_t)(((j / STAGES) & 1) ^ 1));
+      if (elect_one()) {
+        uint8_t* sK = smem + L::KV + st * L::STAGE_BYTES;
+        mbar_arrive_expect_tx(&kv_full[st], 2 * kv_bytes);
+        tma_load_5d(sK, &p.mapK, &kv_full[st], head * D, 0, kvv, yb * p.kh, kv_frame);
+        tma_load_5d(sK + FA_TILE_BYTES, &p.mapV, &kv_full[st], head * D, 0, kvv, yb * p.kh, kv_frame);
+        if (D == 80) {
+          tma_load_5d(sK + 2 * FA_TILE_BYTES, &p.mapKx, &kv_full[st], head * D + 64, 0, kvv, yb * p.kh, kv_frame);
+          tma_load_5d(sK + 2 * FA_TILE_BYTES + L::XB, &p.mapVx, &kv_full[st], head * D + 64, 0, kvv, yb * p.kh, kv_frame);
         }
       }
-      if (pend) issue_pv();
+      if (++yb == p.kv_yblocks) { yb = 0; ++vi; }
     }
-  } else {
-    // ===================== softmax groups: warps 2-5 own tile A, warps 6-9 tile B; thread == query row ==========
-    const int sl = (warp - 2) >> 2;
-    const int lane_grp = warp & 3;                                  // TMEM lane quarter this warp may access
-    const int row = lane_grp * 32 + lane;
-    const uint32_t lane_addr = uint32_t(lane_grp * 32) << 16;
-    const uint32_t tS = tmem_base + lane_addr + sl * L::S_STRIDE;
-    const uint32_t tP = tmem_base + lane_addr + L::P_BASE + sl * L::P_STRIDE;
-    const uint32_t tO = tmem_base + lane_addr + L::O_BASE + sl * L::O_STRIDE;
-    const int nchunk = NCH > 0 ? NCH : p.kv_n / 16;
-    const float c = p.scale_log2;
-    const f32x2 c2 = f2_splat(c);
-
-    // normalise O_t by the row sum and store the 64 channels of this thread's query row (bf16)
-    auto epilogue = [&](int ti, int head, int view, int frame, float l_tot) {
-      const int yy = row / p.qw, xx = row - yy * p.qw;
-      const int x = (ti % p.tiles_x) * p.qw + xx, y = (ti / p.tiles_x) * p.qh + yy;
-      const bool ok = row < p.qw * p.qh && x < p.W && y < p.H;
-      const float inv = 1.f / l_tot;
-      const long long token = (((long long)frame * p.H + y) * p.V + view) * p.W + x;
-      __nv_bfloat16* dst = p.out + token * p.out_ld + head * FA_D;
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        uint32_t o[32];
-        tmem_ld_32x32(tO + hh * 32, o);
-        tmem_ld_wait();
-        if (ok) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            *reinterpret_cast<uint4*>(dst + hh * 32 + i * 8) = make_uint4(
-                pack_bf16x2(__uint_as_float(o[i * 8 + 0]) * inv, __uint_as_float(o[i * 8 + 1]) * inv),
-                pack_bf16x2(__uint_as_float(o[i * 8 + 2]) * inv, __uint_as_float(o[i * 8 + 3]) * inv),
-                pack_bf16x2(__uint_as_float(o[i * 8 + 4]) * inv, __uint_as_float(o[i * 8 + 5]) * inv),
-                pack_bf16x2(__uint_as_float(o[i * 8 + 6]) * inv, __uint_as_float(o[i * 8 + 7]) * inv));
-          }
-        }
-      }
-      if (D == 80) {                  // channels 64..79
-        uint32_t o[16];
-        tmem_ld_32x16(tO + 64, o);
-        tmem_ld_wait();
-        if (ok) {
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            *reinterpret_cast<uint4*>(dst + 64 + i * 8) = make_uint4(
-                pack_bf16x2(__uint_as_float(o[i * 8 + 0]) * inv, __uint_as_float(o[i * 8 + 1]) * inv),
-                pack_bf16x2(__uint_as_float(o[i * 8 + 2]) * inv, __uint_as_float(o[i * 8 + 3]) * inv),
-                pack_bf16x2(__uint_as_float(o[i * 8 + 4]) * inv, __uint_as_float(o[i * 8 + 5]) * inv),
-                pack_bf16x2(__uint_as_float(o[i * 8 + 6]) * inv, __uint_as_float(o[i * 8 + 7]) * inv));
-          }
-        }
-      }
-    };
-
-    // The exp2 phase saturates the MUFU of all four schedulers; the two groups take turns in it (named barriers
-    // 1 = "A may go", 2 = "B may go"), so one group's TMEM traffic, maxima and barrier waits hide behind the other's
-    // exponentials instead of the two running in lock step. Group B hands A the first turn.
-    if (sl == 1 && dbgmode != 4) named_bar_arrive(1, 256);
-    uint32_t n = 0;                  // blocks this group has processed (phase of s_full / pv_done)
-    bool have_prev = false;
-    int prev_ti = 0, prev_head = 0, prev_view = 0, prev_frame = 0;
-    float l_prev = 1.f;
-    for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
-      const FaItem t = fa_decode(p, item);
-      if (sl == 1 && !t.has_b) continue;
-      float m_run = -INFINITY, l_run = 0.f;
-      // turn taking pays off when a tile has several key blocks (view attention: 583 vs 637 us at level 0); with a single
-      // block per tile (text: 77 keys) the hand-over only adds latency (84 vs 73 us)
-      const bool turns = t.has_b && t.nblk > 1 && dbgmode != 4;
-      for (int j = 0; j < t.nblk; ++j, ++n) {
-        const bool tl = dbgmode == 8 && blockIdx.x == 0 && lane_grp == 0 && lane == 0;
-        mbar_wait(&s_full[sl], n & 1);
-        FA_STAMP(tl, sl, n, 0);
-        tc_fence_after();
-        uint32_t sv[8][16];
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch)
-          if (ch < nchunk) tmem_ld_32x16(tS + ch * 16, sv[ch]);
-        tmem_ld_wait();
-        FA_STAMP(tl, sl, n, 1);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_free[sl]);      // the tensor core may overwrite S_t with the next block
-        if (dbgmode == 1) {
-          mbar_wait(&pv_done[sl], (n & 1) ^ 1);
-          tc_fence_after();
-          if (j == 0 && have_prev) epilogue(prev_ti, prev_head, prev_view, prev_frame, l_prev);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&p_full[sl]);
-          l_run = 1.f;
-          continue;
-        }
-        // row maximum: four independent chains per chunk
-        float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) {
-          if (ch < nchunk) {
-#pragma unroll
-            for (int tt = 0; tt < 16; ++tt)
-              if (!MASK || ch * 16 + tt < p.kv_rows) mx4[tt & 3] = fmaxf(mx4[tt & 3], __uint_as_float(sv[ch][tt]));
-          }
-        }
-        const float m_new = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3])) * c;
-        const bool upd = m_new > m_run + FA_LAZY_LOG2;               // always true for the first block (m_run = -inf)
-        const float alpha = upd ? ex2_approx(m_run - m_new) : 1.f;   // first block: exp2(-inf) = 0
-        if (upd) m_run = m_new;
-        const bool need = (j > 0) && __any_sync(0xffffffffu, upd);
-        const f32x2 nm2 = f2_splat(-m_run);
-        f32x2 rs2[2] = {0ull, 0ull};
-        // Per-block rendezvous of the two groups. ptxas sees no dependence between MUFU.EX2 and BAR.SYNC and schedules the
-        // exponentials AHEAD of this barrier, so what the pair of named barriers really does is keep the two groups within
-        // one block of each other (measured: 550 us with it, 637 us free-running at level 0). Forcing the exponentials
-        // behind the barrier (a true alternation of the exp2 phases, r02 experiment) serialises the groups' non-MUFU work
-        // with each other's exponentials and is slower (611 us).
-        FA_STAMP(tl, sl, n, 2);
-        if (turns) named_bar_sync(1 + sl, 256);
-        FA_STAMP(tl, sl, n, 3);
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) {
-          if (ch < nchunk) {
-#pragma unroll
-            for (int tt = 0; tt < 8; ++tt) {
-              const f32x2 xs = f2_fma(f2_pack(__uint_as_float(sv[ch][2 * tt]), __uint_as_float(sv[ch][2 * tt + 1])), c2, nm2);
-              float x0, x1;
-              f2_unpack(xs, x0, x1);
-              float e0 = ex2_approx_ordered(x0), e1 = ex2_approx_ordered(x1);
-              if (MASK) {
-                if (ch * 16 + 2 * tt >= p.kv_rows) e0 = 0.f;
-                if (ch * 16 + 2 * tt + 1 >= p.kv_rows) e1 = 0.f;
-              }
-              rs2[tt & 1] = f2_add(rs2[tt & 1], f2_pack(e0, e1));
-              sv[ch][tt] = pack_bf16x2(e0, e1);        // packed P overwrites the (dead) first half of the chunk
-            }
-          }
-        }
-        {
-          float a0, a1;
-          f2_unpack(f2_add(rs2[0], rs2[1]), a0, a1);
-          const float rs = a0 + a1;
-          // the hand-over must not be scheduled ahead of the exponentials it stands for: its thread count is made to
-          // depend (vacuously — a row sum is never this NaN pattern) on the sum of all of them
-          if (turns) named_bar_arrive(2 - sl, 256u + (__float_as_uint(rs) == 0x7fc0beefu ? 32u : 0u));
-          l_run = l_run * alpha + rs;
-          FA_STAMP(tl && rs >= 0.f, sl, n, 4);
-        }
-        // P_t / O_t may only be touched once the previous PV of this tile slot has retired
-        mbar_wait(&pv_done[sl], (n & 1) ^ 1);
-        FA_STAMP(tl, sl, n, 5);
-        tc_fence_after();
-        if (j == 0) {
-          if (have_prev) epilogue(prev_ti, prev_head, prev_view, prev_frame, l_prev);
-        } else if (need) {
-          // the reference maximum of some row moved: rescale the accumulator in place (alpha = 1 for the other rows)
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            uint32_t o[32];
-            tmem_ld_32x32(tO + hh * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_32x32(tO + hh * 32, o);
-          }
-          if (D == 80) {
-            uint32_t o[16];
-            tmem_ld_32x16(tO + 64, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_32x16(tO + 64, o);
-          }
-        }
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) {
-          if (ch < nchunk) {
-            uint32_t pk[8];
-#pragma unroll
-            for (int tt = 0; tt < 8; ++tt) pk[tt] = sv[ch][tt];
-            tmem_st_32x8(tP + ch * 8, pk);
-          }
-        }
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[sl]);
-        FA_STAMP(tl, sl, n, 6);
-      }
-      have_prev = true;
-      prev_ti = t.t0 + sl; prev_head = t.head; prev_view = t.view; prev_frame = t.frame;
-      l_prev = l_run;
-    }
-    if (sl == 0 && dbgmode != 4) named_bar_sync(1, 256);          // consume the turn that is still outstanding
-    if (have_prev) {
-      mbar_wait(&pv_done[sl], (n & 1) ^ 1);
-      tc_fence_after();
-      epilogue(prev_ti, prev_head, prev_view, prev_frame, l_prev);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // ===================== consumer warpgroups =====================
+  const int wg = warp >> 2;
+  const int quad = lane & 3;
+  const uint32_t base = smem_u32(smem);
+  const uint64_t dQ = wgmma_desc(base + L::Q + wg * 64 * 128, 16, 1024, kSw128);
+  const uint64_t dQx = wgmma_desc(base + L::QX + wg * 64 * 32, 16, 256, kSw32);
+  const uint64_t dK0 = wgmma_desc(base + L::KV, 16, 1024, kSw128);
+  const uint64_t dV0 = wgmma_desc(base + L::KV + FA_TILE_BYTES, 1024, 1024, kSw128);
+  const uint64_t dKx0 = wgmma_desc(base + L::KV + 2 * FA_TILE_BYTES, 16, 256, kSw32);
+  const uint64_t dVx0 = wgmma_desc(base + L::KV + 2 * FA_TILE_BYTES + L::XB, 256, 256, kSw32);
+  constexpr uint64_t STAGE_STEP = L::STAGE_BYTES >> 4;          // start-address field is in 16-byte units
+  const float c = p.scale_log2;
+  const bool mask = p.kv_rows < FA_MAX_KEYS;
+
+  float o[32], ox[8];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) ox[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // rows r and r + 8 of this thread
+
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nblk; ++j) {
+    const int st = j % STAGES;
+    mbar_wait(&kv_full[st], (uint32_t)((j / STAGES) & 1));
+    float s[64];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_ss<128>(s, dQ + 2 * k, dK0 + STAGE_STEP * st + 2 * k, k > 0 ? 1u : 0u);
+    if (D == 80) wgmma_ss<128>(s, dQx, dKx0 + STAGE_STEP * st, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+
+    // scaled logits (log2 domain), padding keys -> -inf; row maximum over the quad
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        float v = s[4 * jj + e] * c;
+        if (mask && 8 * jj + 2 * quad + (e & 1) >= p.kv_rows) v = -INFINITY;
+        s[4 * jj + e] = v;
+        mx[e >> 1] = fmaxf(mx[e >> 1], v);
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      const float m_new = fmaxf(m_run[h], mx[h]);
+      alpha[h] = ex2_approx(m_run[h] - m_new);                  // first block: exp2(-inf) = 0
+      m_run[h] = m_new;
+    }
+    float rs[2] = {0.f, 0.f};
+    uint32_t pa[8][4];                                           // P as the A fragments of 8 K = 16 key steps
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float e0 = ex2_approx(s[4 * jj + 2 * h] - m_run[h]);
+        const float e1 = ex2_approx(s[4 * jj + 2 * h + 1] - m_run[h]);
+        rs[h] += e0 + e1;
+        pa[jj >> 1][(jj & 1) * 2 + h] = pack_bf16x2(e0, e1);
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + rs[h];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[4 * jj + e] *= alpha[e >> 1];
+    }
+    if (D == 80) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) ox[e] *= alpha[(e >> 1) & 1];
+    }
+
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {      // 16 keys per step: 16 rows (128 B each) of V
+      wgmma_rs_tb<64>(o, pa[kk], dV0 + STAGE_STEP * st + kk * (2048 >> 4), 1u);
+      if (D == 80) wgmma_rs_tb<16>(ox, pa[kk], dVx0 + STAGE_STEP * st + kk * (512 >> 4), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    if (D == 80) wgmma_fence_regs(ox);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[st]);   // both of this warpgroup's wgmma groups have retired
+  }
+
+  // normalise by the row sums and store this thread's two query rows (bf16)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.f / l;
+    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    const int yy = row / p.qw, xx = row - yy * p.qw;
+    const int x = (ti % p.tiles_x) * p.qw + xx, y = (ti / p.tiles_x) * p.qh + yy;
+    if (row >= p.qw * p.qh || x >= p.W || y >= p.H) continue;
+    const long long token = (((long long)frame * p.H + y) * p.V + view) * p.W + x;
+    __nv_bfloat16* dst = p.out + token * p.out_ld + head * D + 2 * quad;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+      *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+    if (D == 80) {
+#pragma unroll
+      for (int jj = 0; jj < 2; ++jj)
+        *reinterpret_cast<uint32_t*>(dst + 64 + 8 * jj) = pack_bf16x2(ox[4 * jj + 2 * h] * inv, ox[4 * jj + 2 * h + 1] * inv);
+    }
   }
 }
-
-typedef void (*FaKernel)(const FaParams);
-static FaKernel fa_kernels[10] = {
-    attn_fa_kernel<false, 0, 64>, attn_fa_kernel<false, 2, 64>, attn_fa_kernel<false, 5, 64>, attn_fa_kernel<false, 7, 64>, attn_fa_kernel<false, 8, 64>,
-    attn_fa_kernel<true, 0, 64>,  attn_fa_kernel<true, 2, 64>,  attn_fa_kernel<true, 5, 64>,  attn_fa_kernel<true, 7, 64>,  attn_fa_kernel<true, 8, 64>};
-// head_dim 80 (BASELINE.json configs[4] sweep): the 112-key block of 32x56 views, and the generic chunk count
-static FaKernel fa_kernels80[3] = {attn_fa_kernel<false, 7, 80>, attn_fa_kernel<false, 0, 80>, attn_fa_kernel<true, 0, 80>};
 
 }  // namespace pn
 
@@ -513,7 +257,6 @@ extern "C" int pn_attention(const pn_attn_args* a, void* stream_v) {
   PN_REQUIRE(a->q && a->k && a->v && a->out, "pn_attention: null tensor pointer");
   PN_REQUIRE(a->head_dim == 64 || a->head_dim == 80, "pn_attention: head_dim %d unsupported (64 or 80)", a->head_dim);
   const int FA_D = a->head_dim;
-  const int max_keys = FA_D == 80 ? 112 : 128;      // head_dim 80: S 2 x 112 + P 2 x 56 + O 2 x 80 tensor-memory columns
   PN_REQUIRE(a->heads > 0 && a->F > 0 && a->H > 0 && a->V > 0 && a->V <= 8 && a->W > 0, "pn_attention: bad query geometry");
   PN_REQUIRE(a->Hk > 0 && a->Vk > 0 && a->Vk <= 8 && a->Wk > 0 && a->kv_frame_div > 0, "pn_attention: bad key geometry");
   PN_REQUIRE(a->q_ld % 8 == 0 && a->kv_ld % 8 == 0 && a->out_ld % 8 == 0, "pn_attention: token strides must be multiples of 8");
@@ -532,15 +275,13 @@ extern "C" int pn_attention(const pn_attn_args* a, void* stream_v) {
   p.tiles_x = (int)((a->W + p.qw - 1) / p.qw);
   p.tiles_y = (int)((a->H + p.qh - 1) / p.qh);
   // key block: full key-view width (must fit one block row-wise), rows = largest divisor of Hk with <= 128 keys
-  PN_REQUIRE(a->Wk <= 128, "pn_attention: key view width %lld > 128 unsupported", (long long)a->Wk);
+  PN_REQUIRE(a->Wk <= FA_MAX_KEYS, "pn_attention: key view width %lld > %d unsupported", (long long)a->Wk, FA_MAX_KEYS);
   p.kw = (int)a->Wk;
-  PN_REQUIRE(p.kw <= max_keys, "pn_attention: key view width %lld > %d unsupported at head_dim %d", (long long)a->Wk, max_keys, FA_D);
-  int kh = max_keys / p.kw;
+  int kh = FA_MAX_KEYS / p.kw;
   if (kh > a->Hk) kh = (int)a->Hk;
   while (kh > 1 && (a->Hk % kh) != 0) --kh;
   p.kh = kh;
   p.kv_rows = p.kw * p.kh;
-  p.kv_n = (p.kv_rows + 15) / 16 * 16;
   p.kv_yblocks = (int)(a->Hk / p.kh);
   for (int v = 0; v < a->V; ++v) {
     const int cnt = a->kv_view_count[v];
@@ -553,13 +294,6 @@ extern "C" int pn_attention(const pn_attn_args* a, void* stream_v) {
   }
   p.kv_frame_div = a->kv_frame_div;
   p.scale_log2 = a->scale * 1.4426950408889634f;
-#ifdef PN_GEMM_ROLE_TIMERS
-  {
-    static int dbg = -1;
-    if (dbg < 0) { const char* e = std::getenv("PN_ATTN_DEBUG"); dbg = e ? std::atoi(e) : 0; }
-    p.debug = dbg;
-  }
-#endif
   p.out = reinterpret_cast<__nv_bfloat16*>(a->out);
   p.out_ld = a->out_ld;
 
@@ -596,30 +330,14 @@ extern "C" int pn_attention(const pn_attn_args* a, void* stream_v) {
     }
   }
   p.tiles_per_group = p.tiles_x * p.tiles_y;
-  p.pairs = (p.tiles_per_group + 1) / 2;
-  const long long items = (long long)p.pairs * a->heads * a->V * a->F;
+  const long long items = (long long)p.tiles_per_group * a->heads * a->V * a->F;
   PN_REQUIRE(items > 0 && items < (1ll << 31), "pn_attention: too many query tiles");
-  p.total_items = (int)items;
-  const int grid = items < sm_count() ? (int)items : sm_count();
-  const int nch = p.kv_n / 16;
-  const int slot = nch == 8 ? 4 : nch == 7 ? 3 : nch == 5 ? 2 : nch == 2 ? 1 : 0;
-  const bool masked = p.kv_rows < p.kv_n;
-  const FaKernel kern = FA_D == 80 ? fa_kernels80[masked ? 2 : (nch == 7 ? 0 : 1)] : fa_kernels[(masked ? 5 : 0) + slot];
+  void (*kern)(FaParams) = FA_D == 80 ? attn_fa_kernel<80> : attn_fa_kernel<64>;
   const size_t smem_total = FA_D == 80 ? FaL<80>::TOTAL : FaL<64>::TOTAL;
   {
     const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem_total);
     if (rc != PN_OK) return rc;
   }
-  PN_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(FA_THREADS), smem_total, reinterpret_cast<cudaStream_t>(stream_v), 1, p));
+  PN_CHECK_CUDA(launch_kernel(kern, dim3((unsigned)items), dim3(FA_THREADS), smem_total, reinterpret_cast<cudaStream_t>(stream_v), 1, p));
   return PN_OK;
 }
-
-#ifdef PN_GEMM_ROLE_TIMERS
-// diagnostics (not part of the product ABI): the timeline of CTA 0 of the last pn_attention launch made with PN_ATTN_DEBUG=8
-extern "C" int pn_debug_attn_timeline(long long* out, int n) {
-  PN_CHECK_CUDA(cudaDeviceSynchronize());
-  const size_t bytes = sizeof(long long) * (size_t)(n < 3 * pn::FA_TL_BLOCKS * 8 ? n : 3 * pn::FA_TL_BLOCKS * 8);
-  PN_CHECK_CUDA(cudaMemcpyFromSymbol(out, pn::g_fa_tl, bytes));
-  return PN_OK;
-}
-#endif

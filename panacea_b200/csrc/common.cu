@@ -171,14 +171,13 @@ int sm_count() {
   if (g_sm_count[dev] == 0) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    g_sm_count[dev] = n > 0 ? n : 148;
+    g_sm_count[dev] = n > 0 ? n : 132;
   }
   return g_sm_count[dev];
 }
 
 bool pdl_enabled() {
-  // measured on B200 (r02_bench2_pdl / r02_bench2_nopdl): 114.1 ms per step with it, 112.8 ms without — the 1.3 k launches of
-  // the captured graph are not launch-latency bound, so it is opt-in (PN_PDL=1)
+  // opt-in (PN_PDL=1): the launches of the captured step graph are not launch-latency bound
   static const bool on = [] { const char* e = std::getenv("PN_PDL"); return e && std::atoi(e) != 0; }();
   return on;
 }

@@ -1,4 +1,4 @@
-// tcgen05 GEMM / implicit-GEMM convolution for sm_100a.
+// wgmma GEMM / implicit-GEMM convolution for sm_90a.
 //
 //   out[row, n] = epilogue( sum_{tap, c} A[pixel(row) + tap][c] * Wt[n][tap * C + c] )
 //
@@ -7,44 +7,27 @@
 // Conv1d) are coordinate offsets of the same map, so im2col never exists in memory and the conv zero
 // padding is TMA's out-of-bounds zero fill (outer panorama border only, reference: openaimodel.py:413,
 // 455-462 Conv2d(padding=1) on the width-concatenated 6-view image; :418,468-476 Conv1d(k=3,padding=1)).
-// B is the packed weight matrix [N, taps*C] (K-major, bf16). Accumulation is fp32 in TMEM.
+// B is the packed weight matrix [N, taps*C] (K-major, bf16). Accumulation is fp32 in registers.
 //
-// Kernel structure (persistent, one CTA per SM, 320 or 448 threads):
-//   warp 0     : TMA producer  (A box [tn,th,tw,64] + B box [BN,64] per k-block, 128B swizzle)
-//   warp 1     : TMEM alloc + UMMA issuer (tcgen05.mma cta_group::1 kind::f16, M=128, N=BN, K=16)
-//   warps 2..  : epilogue (residual prefetch; tcgen05.ld -> bias/row-vector/GEGLU -> smem transpose -> +residual -> global)
-// Pipelines: smem full/empty ring (TMA<->MMA) and a 2-deep TMEM accumulator ring (MMA<->epilogue) so the
-// epilogue of tile i overlaps the main loop of tile i+1.
+// Kernel structure (one CTA per 128 x BN output tile, 288 threads):
+//   warps 0-3, 4-7 : two consumer warpgroups, 64 tile rows each: wgmma m64nBNk16 from the shared-memory ring,
+//                    then the epilogue straight from the accumulator registers (bias / row vector / LayerNorm fold /
+//                    GEGLU / residuals -> global)
+//   warp 8         : TMA producer (A box [tn,th,tw,64] + B box [BN,64] per k-block, 128B swizzle)
+// Pipeline: STAGES-deep full/empty mbarrier ring; a stage is handed back once the wgmma group that read it retired.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/panacea_b200.h"
-
-#include <cstdlib>
 
 namespace pn {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle atom row
-// warp 0 TMA, warp 1 MMA, warps 2.. epilogue: 8 warps for the fp32/residual mode (168 registers each), 12 for the
-// ALU-heavy bf16 / GEGLU modes (the register file is granted per 4-warp group: 16 warps x 128 registers)
-// streaming epilogues: 4 = fp32, 5 = bf16, 7 = bf16 that also emits the rows' (sum, sum of squares) — a PRODUCER of the
-// bf16 token stream —, 8 = bf16 whose A operand is the un-normalised token stream: it finishes a folded LayerNorm in the
-// epilogue (a CONSUMER). 7 and 8 are separate instantiations so that the plain kernels carry none of their code.
-constexpr bool gemm_streaming(int mode) { return mode == 4 || mode == 5 || mode == 7 || mode == 8; }
-constexpr bool gemm_stream_bf16(int mode) { return mode == 5 || mode == 7 || mode == 8; }
-constexpr int gemm_threads(int mode) { return (mode == 0 || mode == 3 || mode == 6) ? 320 : gemm_streaming(mode) ? 352 : mode == 2 ? 576 : 448; }
+constexpr int GEMM_THREADS = 288;
 
 struct GemmParams {
   CUtensorMap mapA;
   CUtensorMap mapB;
-  CUtensorMap mapOut;          // MODE 4 only: fp32 output / residual, box {32 floats, 128 rows}
-  CUtensorMap mapRes;
-  int has_res;
-#ifdef PN_GEMM_ROLE_TIMERS
-  int debug;                   // diagnostics builds only — PN_GEMM_DEBUG timing experiments: 1 = no TMA loads after the first
-                               // ring fill, 2 = no MMA issue, 3 = epilogue reads TMEM only, 4 = no global stores, 5 = role timers,
-                               // 6 = 2 + 3 (loads only), 7 = 1 + 3 (MMAs only); +8 = the experiment with the role timers on
-#endif
   // geometry of the A tensor / output rows
   int NB, H, W;
   int tw, th, tn;             // tile box extents, tw*th*tn == 128
@@ -56,913 +39,236 @@ struct GemmParams {
   void* out;
   const float* bias;
   const float* rowvec;
-  const float* residual;
+  const void* residual;
   const float* residual2;
   long long ldo, ldr, ldr2, ldv;
   int rows_per_group, n_groups;
   // LayerNorm folded into the GEMMs around the bf16 token stream (attention.py:726-747: x + attn(norm(x))):
-  //  * a PRODUCER of the stream (MODE 5) also emits per-row partial sums (sum, sum of squares) of the bf16 values it
-  //    stores: ln_stats_out[row][tile_col * 2 + half][2] (ln_parts_out = 2 * tiles_col);
-  //  * a CONSUMER (MODE 5 or 2) multiplies the UN-normalised stream by W' = W diag(gamma) and finishes the LayerNorm in
-  //    its epilogue: out = rstd_m * (acc - mean_m * s_n) + t_n, s_n = sum_k W'[n,k], t_n = sum_k beta_k W[n,k] (+ bias,
+  //  * a PRODUCER of the stream also emits per-row partial sums (sum, sum of squares) of the values it stores:
+  //    ln_stats_out[row][tile_col * 2 + half][2] (ln_parts_out = 2 * tiles_col, half = which half of the tile's columns);
+  //  * a CONSUMER multiplies the UN-normalised stream by W' = W diag(gamma) and finishes the LayerNorm in its
+  //    epilogue: out = rstd_m * (acc - mean_m * s_n) + t_n, s_n = sum_k W'[n,k], t_n = sum_k beta_k W[n,k] (+ bias,
   //    passed as `bias`), mean/rstd from the ln_parts_in partial sums of row m.
   const float* ln_stats_in;
   const float* ln_colsum;
   float* ln_stats_out;
   int ln_parts_in, ln_parts_out;
   float ln_inv_dim, ln_eps;
-  int out_bf16;
   int res_bf16;                // the residual is bf16 (bf16 token stream of the transformer blocks), bf16 output only
-  int geglu;
-  int bstat;                   // weight-stationary schedule (K = 5 k-blocks, taps = 1): see gemm_tc_kernel
 };
 
-template <int BN, int STAGES, int NCTA, int MODE>
+template <int BN, int STAGES>
 struct GemmSmem {
-  static constexpr int NEPI = gemm_streaming(MODE) ? 8 : gemm_threads(MODE) / 32 - 2;
-  static constexpr int STAGE_WARP_BYTES = (MODE == 0 || MODE == 3 || MODE == 6) ? 4096 : 2048;   // 32 rows x (128 | 64) B
-  // MODE 6 (haloed 3x3 conv): A ring of HALO_STAGES haloed tiles [(16+2) x (8+2) pixels x 64 ch], B ring of STAGES weight tiles
-  static constexpr int HALO_STAGES = 3;
-  static constexpr int A_HALO_BYTES = 23552;             // 18*10*128 = 23040, padded to a multiple of 1024
-  static constexpr int A_HALO_TX = 18 * 10 * 128;
-  static constexpr int RCHUNK_BYTES = gemm_stream_bf16(MODE) ? 128 * 64 : 128 * 128;              // 128 rows x 32 (bf16 | fp32)
   static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = (BN / NCTA) * BK * 2;   // a CTA pair splits the N tile: each CTA stages BN/2 weight rows
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int RING_BYTES = MODE == 6 ? HALO_STAGES * A_HALO_BYTES + STAGES * B_BYTES : STAGES * STAGE_BYTES;
-  static constexpr int STAGING_BYTES = gemm_streaming(MODE) ? (BN / 32) * RCHUNK_BYTES : NEPI * STAGE_WARP_BYTES;
-  static constexpr bool BIAS_SMEM = (MODE == 1 || MODE == 2);    // the ALU-bound epilogues stage their bias slice in smem
-  static constexpr int ROWMAP_BYTES = gemm_streaming(MODE) ? 0 : NEPI * 32 * 4 + (BIAS_SMEM ? NEPI * 512 : 0);
-  static constexpr int BAR_BYTES = (2 * STAGES + 4 + 2 * (BN / 32) + 8) * 8 + 16;
-  static constexpr int TOTAL = RING_BYTES + STAGING_BYTES + ROWMAP_BYTES + BAR_BYTES + 1024;
+  static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;   // a multiple of 1024: every tile starts on a swizzle atom
+  static constexpr int TOTAL = STAGES * STAGE_BYTES + 2 * STAGES * 8 + 1024;
 };
 
-// MODE: 0 = fp32 store (+ one fp32 residual), 1 = bf16 store, 2 = GEGLU (bf16 store of N/2 columns),
-//       3 = fp32 store + two fp32 residuals (kept apart so that mode 0 does not carry its registers),
-//       4 = streaming fp32 epilogue for tiles whose 128 rows are consecutive output rows: the fp32 residual tile is
-//           TMA-loaded into a swizzled shared-memory tile ahead of time, the epilogue warps update it in place
-//           (thread == row, conflict-free), and a dedicated warp TMA-stores it — no global LD/ST instruction and no
-//           register prefetch in the epilogue warps. Used for the HBM-bound K<=1280 linears and the temporal conv.
-//       5 = the same streaming epilogue with a bf16 store and no residual (q/k/v and query projections).
-//       6 = 3x3 conv with a HALOED A tile: the 9 taps of one 64-channel chunk are 9 row-shifted UMMA views of ONE
-//           (16+2)x(8+2)-pixel tile in shared memory, so the activations cross the L2->SM fabric once instead of 9
-//           times (the L2-bound N=160 tile of the level-0/1 convs); fp32 store through the generic epilogue.
-// Role cycle accounting of CTA 0 (tools/gemm_probe3.py prints it): compiled in only with -DPN_GEMM_ROLE_TIMERS
-// (PN_GEMM_ROLE_TIMERS=1 python -m panacea_b200.build --force), then enabled at run time by PN_GEMM_DEBUG=5
-//  [0] issuer total  [1] issuer waiting accumulator  [2] issuer waiting operands  [3] tiles
-//  [4] producer total [5] producer waiting free slots
-//  [6] epilogue warp 2 total [7] waiting tmem_full [8] waiting staging chunk  [9] store warp waiting chunks [10] waiting smem reads
-__device__ unsigned long long g_gemm_dbg[16];
-#ifdef PN_GEMM_ROLE_TIMERS
-constexpr bool kRoleTimers = true;
-#else
-constexpr bool kRoleTimers = false;
-#endif
-// The PN_GEMM_DEBUG timing experiments (1-5) exist only in diagnostics builds
-// (PN_GEMM_ROLE_TIMERS=1 python -m panacea_b200.build --force); in the product build `dbgmode` is the constant 0.
-
-template <int BN, int STAGES, int NCTA, int MODE>
-__global__ void __launch_bounds__(gemm_threads(MODE), 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
-  using S = GemmSmem<BN, STAGES, NCTA, MODE>;
-  constexpr int NEPI = S::NEPI;
-  constexpr int EG = NEPI / 4;                 // epilogue warps per TMEM lane quarter
+// MODE: 0 = fp32 store (+ fp32 residual, + second fp32 residual), 1 = bf16 store (+ fp32 or bf16 residual, LayerNorm
+// fold / row statistics), 2 = GEGLU (bf16 store of N/2 columns)
+template <int BN, int STAGES, int MODE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
+  using S = GemmSmem<BN, STAGES>;
+  constexpr int NJ = BN / 8;                   // 8-column accumulator blocks per thread row
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
-  uint8_t* stage_base = smem;
-  uint8_t* staging = smem + S::RING_BYTES;
-  int* rowmap = reinterpret_cast<int*>(staging + S::STAGING_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(rowmap) + S::ROWMAP_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;       // [2]
-  uint64_t* r_full = tmem_empty + 2;          // [BN/32]  MODE 4: tile chunk holds the residual / is free for the epilogue
-  uint64_t* c_ready = r_full + BN / 32;       // [BN/32]  MODE 4: chunk updated by its 4 epilogue warps -> store it
-  uint64_t* a_full = c_ready + BN / 32;       // [3]      MODE 6: haloed A tiles
-  uint64_t* a_empty = a_full + 4;             // [3]
-  uint64_t* b_full = a_full;                  // [5]      weight-stationary: resident weight k-blocks (modes other than 6)
-  uint64_t* b_empty = a_empty + 1;            // [1]      ... all MMAs reading them have retired
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(a_empty + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-#ifdef PN_GEMM_ROLE_TIMERS
-  const int dbgmode = p.debug & 7;      // the experiment
-  const bool dbgtime = (p.debug & 8) != 0 || (p.debug & 7) == 5;   // role timers of CTA 0 (5 = timers alone, 8+n = experiment n timed)
-#else
-  constexpr int dbgmode = 0;
-  constexpr bool dbgtime = false;
-#endif
-  // NCTA == 2: the two CTAs of a cluster form a UMMA pair (cta_group::2). Each CTA owns 128 rows of a 256-row
-  // tile (its own A stage and TMEM lanes) and stages half of the N tile's weight rows; the leader (rank 0)
-  // issues the MMAs for both, and the weights cross the L2->SM fabric once per pair instead of once per CTA.
-  const uint32_t cta_rank = (NCTA == 2) ? cluster_ctarank() : 0u;
-  const int unit = (NCTA == 2) ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;          // persistent scheduling unit
-  const int num_units = (NCTA == 2) ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-
+  // column tile fastest: the CTAs that run together share an A tile in L2
+  const int tcol = blockIdx.x % p.tiles_col;
+  int tm = blockIdx.x / p.tiles_col;
+  const int twi = tm % p.tiles_w; tm /= p.tiles_w;
+  const int thi = tm % p.tiles_h;
+  const int tni = tm / p.tiles_h;
   const int num_k_blocks = p.taps_h * p.taps_w * p.kc_per_tap;
-  const int tiles_m = p.tiles_w * p.tiles_h * p.tiles_n;
-  const int tiles_m_units = (tiles_m + NCTA - 1) / NCTA;
-  const int num_tiles = tiles_m_units * p.tiles_col;
-  // Tile schedule. Default: tile = unit + i * num_units, column tile fastest (concurrent units share an A tile in L2).
-  // Weight-stationary (p.bstat, the K = 320 linears of level 0 whose k loop is only 5 blocks long and L2->SM bound):
-  // unit u keeps ONE column tile (u mod tiles_col) for the whole launch — its weight tile (all 5 k-blocks, parked in
-  // the B halves of ring stages 0..4) is loaded once — and walks a contiguous range of row tiles; the tiles_col units
-  // of a row range advance together, so they still share each A tile in L2. Per k-block only the 16 KB A tile crosses
-  // the L2->SM fabric instead of A + B. (num_units mod tiles_col units stay idle.)
-  int t_begin, t_step, t_count;
-  if (p.bstat) {
-    const int ranges = num_units / p.tiles_col;
-    const int col = unit % p.tiles_col, r = unit / p.tiles_col;
-    const int per = tiles_m_units / ranges, rem = tiles_m_units % ranges;
-    t_begin = col * tiles_m_units + r * per + (r < rem ? r : rem);      // column-major tile index
-    t_count = r < ranges ? per + (r < rem ? 1 : 0) : 0;
-    t_step = 1;
-  } else {
-    t_begin = unit;
-    t_step = num_units;
-    t_count = unit < num_tiles ? (num_tiles - unit + num_units - 1) / num_units : 0;
-  }
-  auto tile_col = [&](int tile) { return p.bstat ? tile / tiles_m_units : tile % p.tiles_col; };
-  auto tile_mu = [&](int tile) { return p.bstat ? tile % tiles_m_units : tile / p.tiles_col; };
-  constexpr uint32_t TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  static_assert(2 * BN <= 512, "two accumulator stages must fit TMEM");
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.mapA);
     tma_prefetch_desc(&p.mapB);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], NEPI * NCTA);  // one arrive per epilogue warp (of both CTAs of a pair)
-    }
-    if (MODE == 6) {
-      for (int i = 0; i < S::HALO_STAGES; ++i) {
-        mbar_init(&a_full[i], 1);
-        mbar_init(&a_empty[i], 1);
-      }
-    } else {
-      for (int i = 0; i < 5; ++i) mbar_init(&b_full[i], 1);
-      mbar_init(b_empty, 1);
-    }
-    if (gemm_streaming(MODE)) {
-      tma_prefetch_desc(&p.mapOut);
-      if (p.has_res) tma_prefetch_desc(&p.mapRes);
-      for (int i = 0; i < BN / 32; ++i) {
-        mbar_init(&r_full[i], 1);
-        mbar_init(&c_ready[i], 4);
-      }
+      mbar_init(&empty_bar[i], 2);             // one arrive per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if (NCTA == 2) tmem_alloc_2sm(tmem_ptr_smem, TMEM_COLS);
-    else tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-  }
-  tc_fence_before();
-  if (NCTA == 2) cluster_sync_all();
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_prologue_done();        // barriers / TMEM are set up: from here on global memory is touched
+  __syncthreads();
+  pdl_prologue_done();        // barriers are set up: from here on global memory is touched
 
-  // Producer and issuer loops are executed by all 32 lanes of their warp with the asynchronous instructions under an
-  // elect.sync predicate: ptxas then emits the TMA / UMMA instructions straight from uniform registers. (Issued from
-  // a `lane == 0` branch every one of them is wrapped in an elect/vote loop, and the single-thread instruction stream
-  // — not the tensor core — set the pace: ~145 cycles per UMMA whatever its N, measured with tools/mma_probe.py
-  // against 64 cycles for N = 128 in tools/ubench/umma_rate.cu.)
-  if (warp == 0 && MODE == 6) {
-    // ===================== MODE 6 producer: one haloed A tile per 64-channel chunk, nine weight tiles per chunk ==========
-    uint8_t* ringA = stage_base;
-    uint8_t* ringB = stage_base + S::HALO_STAGES * S::A_HALO_BYTES;
-    int sa = 0, sb = 0;
-    uint32_t pa = 0, pb = 0;
-    for (int ti = 0, tile = t_begin; ti < t_count; ++ti, tile += t_step) {
-      const int tcol = tile_col(tile);
-      int tm = tile_mu(tile) * NCTA + (int)cta_rank;
-      const int twi = tm % p.tiles_w; tm /= p.tiles_w;
-      const int thi = tm % p.tiles_h; tm /= p.tiles_h;
-      const int x0 = twi * p.tw, y0 = thi * p.th, n0 = tm * p.tn;
-      const int bn0 = tcol * BN + (NCTA == 2 ? (int)cta_rank * (BN / 2) : 0);
-      for (int kc = 0; kc < p.kc_per_tap; ++kc) {
-        mbar_wait(&a_empty[sa], pa ^ 1);
-        if (elect_one()) {
-          if (NCTA == 2) {
-            if (cta_rank == 0) mbar_arrive_expect_tx(&a_full[sa], 2 * S::A_HALO_TX);
-            tma_load_4d_2sm(ringA + sa * S::A_HALO_BYTES, &p.mapA, &a_full[sa], kc * BK, x0 - 1, y0 - 1, n0);
-          } else {
-            mbar_arrive_expect_tx(&a_full[sa], S::A_HALO_TX);
-            tma_load_4d(ringA + sa * S::A_HALO_BYTES, &p.mapA, &a_full[sa], kc * BK, x0 - 1, y0 - 1, n0);
-          }
-        }
-        if (++sa == S::HALO_STAGES) { sa = 0; pa ^= 1; }
-        int kcol = kc * BK;                               // weight column of (tap 0, chunk kc); one tap = C columns
-        for (int tap = 0; tap < 9; ++tap, kcol += p.kc_per_tap * BK) {
-          mbar_wait(&empty_bar[sb], pb ^ 1);
-          if (elect_one()) {
-            uint8_t* sB = ringB + sb * S::B_BYTES;
-            if (NCTA == 2) {
-              if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[sb], 2 * S::B_BYTES);
-              tma_load_2d_2sm(sB, &p.mapB, &full_bar[sb], kcol, bn0);
-            } else {
-              mbar_arrive_expect_tx(&full_bar[sb], S::B_BYTES);
-              tma_load_2d(sB, &p.mapB, &full_bar[sb], kcol, bn0);
-            }
-          }
-          if (++sb == STAGES) { sb = 0; pb ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1 && MODE == 6) {
-    // ===================== MODE 6 UMMA issuer: tap (dy,dx) = the A view shifted by dy*(tw+2)+dx rows ==========
-    if (cta_rank == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM * NCTA, BN, 0, 0);
-      const uint32_t ringA = smem_u32(stage_base);
-      const uint32_t ringB = ringA + S::HALO_STAGES * S::A_HALO_BYTES;
-      // A view: 16 groups of 8 pixels, one image row (8+2 pixels, 1280 B) apart; base offset 0 (the 128B swizzle is
-      // a function of the absolute shared-memory address — verified on B200)
-      const uint64_t descA0 = umma_smem_desc(ringA, 16, 1280);
-      const uint64_t descB0 = umma_smem_desc(ringB, 16, 1024);
-      int sa = 0, sb = 0, acc = 0;
-      uint32_t pa = 0, pb = 0, acc_phase = 0;
-      for (int ti = 0, tile = t_begin; ti < t_count; ++ti, tile += t_step) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kc = 0; kc < p.kc_per_tap; ++kc) {
-          mbar_wait(&a_full[sa], pa);
-          const uint64_t da_tile = descA0 + (uint64_t)(S::A_HALO_BYTES >> 4) * sa;
-#pragma unroll
-          for (int tap = 0; tap < 9; ++tap) {
-            mbar_wait(&full_bar[sb], pb);
-            tc_fence_after();
-            if (elect_one()) {
-              const uint64_t da = da_tile + (uint64_t)(((tap / 3) * 10 + (tap % 3)) * 8);    // rows * 128 B / 16
-              const uint64_t db = descB0 + (uint64_t)(S::B_BYTES >> 4) * sb;
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                const uint32_t accum = (kc > 0 || tap > 0 || k > 0) ? 1u : 0u;
-                if (NCTA == 2) umma_f16_ss_2sm(d_tmem, da + 2 * k, db + 2 * k, idesc, accum);
-                else umma_f16_ss(d_tmem, da + 2 * k, db + 2 * k, idesc, accum);
-              }
-              const bool last = (kc == p.kc_per_tap - 1) && (tap == 8);
-              if (NCTA == 2) {
-                umma_commit_2sm(&empty_bar[sb], 3);
-                if (tap == 8) umma_commit_2sm(&a_empty[sa], 3);
-                if (last) umma_commit_2sm(&tmem_full[acc], 3);
-              } else {
-                umma_commit(&empty_bar[sb]);
-                if (tap == 8) umma_commit(&a_empty[sa]);
-                if (last) umma_commit(&tmem_full[acc]);
-              }
-            }
-            if (++sb == STAGES) { sb = 0; pb ^= 1; }
-          }
-          if (++sa == S::HALO_STAGES) { sa = 0; pa ^= 1; }
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp == 0) {
-    // ===================== TMA producer (every CTA loads its own A rows and its share of B) =====================
+  if (warp == 8) {
+    // ===================== TMA producer (warp-wide loop, TMA issue under elect.sync) =====================
+    const int x0 = twi * p.tw, y0 = thi * p.th, n0 = tni * p.tn;
+    const int bn0 = tcol * BN;
     int stage = 0;
     uint32_t phase = 0;
-    bool first = true;
-    int cur_col = -1;
-    uint32_t bgen = 0;                            // weight-stationary: weight tiles loaded so far
-    const bool dbg = kRoleTimers && dbgtime && blockIdx.x == 0;
-    long long d_t0 = dbg ? clock64() : 0, d_wait = 0;
-    for (int ti = 0, tile = t_begin; ti < t_count; ++ti, tile += t_step) {
-      const int tcol = tile_col(tile);
-      int tm = tile_mu(tile) * NCTA + (int)cta_rank;
-      const int twi = tm % p.tiles_w; tm /= p.tiles_w;
-      const int thi = tm % p.tiles_h; tm /= p.tiles_h;
-      const int tni = tm;                       // >= tiles_n for the odd tail of a pair: fully OOB -> zero fill
-      const int x0 = twi * p.tw, y0 = thi * p.th, n0 = tni * p.tn;
-      const int bn0 = tcol * BN + (NCTA == 2 ? (int)cta_rank * (BN / 2) : 0);
-      if (MODE != 6 && p.bstat && tcol != cur_col) {
-        // new column tile: once every MMA that reads the resident weight tile has retired, replace all its k-blocks
-        if (bgen > 0) mbar_wait(b_empty, (bgen - 1) & 1);
-        if (elect_one()) {
-          for (int kb = 0; kb < num_k_blocks; ++kb) {
-            uint8_t* sB = stage_base + kb * S::STAGE_BYTES + S::A_BYTES;
-            if (NCTA == 2) {
-              if (cta_rank == 0) mbar_arrive_expect_tx(&b_full[kb], 2 * S::B_BYTES);
-              tma_load_2d_2sm(sB, &p.mapB, &b_full[kb], kb * BK, bn0);
-            } else {
-              mbar_arrive_expect_tx(&b_full[kb], S::B_BYTES);
-              tma_load_2d(sB, &p.mapB, &b_full[kb], kb * BK, bn0);
-            }
-          }
-        }
-        cur_col = tcol;
-        ++bgen;
+    int kc = 0, dx = -p.pad_w, dy = -p.pad_h;   // k-block -> (tap row, tap column, channel chunk), kept incrementally
+    for (int kb = 0; kb < num_k_blocks; ++kb) {
+      mbar_wait(&empty_bar[stage], phase ^ 1);
+      if (elect_one()) {
+        uint8_t* sA = smem + stage * S::STAGE_BYTES;
+        mbar_arrive_expect_tx(&full_bar[stage], S::STAGE_BYTES);
+        tma_load_4d(sA, &p.mapA, &full_bar[stage], kc * BK, x0 + dx, y0 + dy, n0);
+        tma_load_2d(sA + S::A_BYTES, &p.mapB, &full_bar[stage], kb * BK, bn0);
       }
-      int kc = 0, dx = -p.pad_w, dy = -p.pad_h;   // k-block -> (tap row, tap column, channel chunk), kept incrementally
-      for (int kb = 0; kb < num_k_blocks; ++kb) {
-        if (!((dbgmode == 1 || dbgmode == 7) && !(first && kb < STAGES))) {   // experiment 1: the ring is filled once, never again
-          { const long long w0 = dbg ? clock64() : 0; mbar_wait(&empty_bar[stage], phase ^ 1); if (dbg) d_wait += clock64() - w0; }
-          if (elect_one()) {
-            uint8_t* sA = stage_base + stage * S::STAGE_BYTES;
-            uint8_t* sB = sA + S::A_BYTES;
-            const uint32_t tx = (MODE != 6 && p.bstat) ? S::A_BYTES : S::STAGE_BYTES;
-            if (NCTA == 2) {
-              if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * tx);   // bytes of both CTAs
-              tma_load_4d_2sm(sA, &p.mapA, &full_bar[stage], kc * BK, x0 + dx, y0 + dy, n0);
-              if (!(MODE != 6 && p.bstat)) tma_load_2d_2sm(sB, &p.mapB, &full_bar[stage], kb * BK, bn0);
-            } else {
-              mbar_arrive_expect_tx(&full_bar[stage], tx);
-              tma_load_4d(sA, &p.mapA, &full_bar[stage], kc * BK, x0 + dx, y0 + dy, n0);
-              if (!(MODE != 6 && p.bstat)) tma_load_2d(sB, &p.mapB, &full_bar[stage], kb * BK, bn0);
-            }
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (++kc == p.kc_per_tap) {
-          kc = 0;
-          if (++dx > p.taps_w - 1 - p.pad_w) { dx = -p.pad_w; ++dy; }
-        }
-      }
-      first = false;
-    }
-    if (dbg && lane == 0) { g_gemm_dbg[4] = (unsigned long long)(clock64() - d_t0); g_gemm_dbg[5] = (unsigned long long)d_wait; }
-  } else if (warp == 1) {
-    // ===================== UMMA issuer (leader CTA of a pair only) =====================
-    // Kept deliberately plain (runtime ring position, descriptors = uniform base + stage * step + k): in this form ptxas
-    // keeps every operand in uniform registers; unrolling by the ring position made it hoist 8 x STAGES descriptors into
-    // vector registers and pay an R2UR per operand per MMA.
-    if (cta_rank == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM * NCTA, BN, 0, 0);
-      const uint64_t descA0 = umma_smem_desc(smem_u32(stage_base), 16, 1024);
-      const uint64_t descB0 = umma_smem_desc(smem_u32(stage_base) + S::A_BYTES, 16, 1024);
-      constexpr uint64_t STAGE_STEP = S::STAGE_BYTES >> 4;      // start-address field is in 16-byte units
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      bool first = true;
-      int cur_col = -1;
-      uint32_t bgen = 0;
-      const bool dbg = kRoleTimers && dbgtime && blockIdx.x == 0;
-      long long d_t0 = dbg ? clock64() : 0, d_acc = 0, d_full = 0;
-      for (int ti = 0, tile = t_begin; ti < t_count; ++ti, tile += t_step) {
-        const bool bstat = MODE != 6 && p.bstat;
-        const int tcol = tile_col(tile);
-        const bool new_b = bstat && tcol != cur_col;              // first tile on a freshly loaded weight tile
-        if (new_b) { cur_col = tcol; ++bgen; }
-        const bool last_b = bstat && (ti + 1 == t_count || tile_col(tile + t_step) != tcol);
-        { const long long w0 = dbg ? clock64() : 0; mbar_wait(&tmem_empty[acc], acc_phase ^ 1); if (dbg) d_acc += clock64() - w0; }
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          const long long w1 = dbg ? clock64() : 0;
-          if (!((dbgmode == 1 || dbgmode == 7) && !(first && kb < STAGES))) mbar_wait(&full_bar[stage], phase);
-          if (dbg) d_full += clock64() - w1;
-          if (new_b) mbar_wait(&b_full[kb], (bgen - 1) & 1);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint64_t da = descA0 + STAGE_STEP * stage;
-            const uint64_t db = descB0 + STAGE_STEP * (bstat ? kb : stage);
-            if ((dbgmode != 2 && dbgmode != 6)) {
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                if (NCTA == 2) umma_f16_ss_2sm(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                else umma_f16_ss(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-              }
-            }
-            // commit: frees the smem slot (in both CTAs) once the MMAs retire; the last one also publishes the tile
-            const bool last_kb = kb == num_k_blocks - 1;
-            if (NCTA == 2) {
-              umma_commit_2sm(&empty_bar[stage], 3);
-              if (last_kb) umma_commit_2sm(&tmem_full[acc], 3);
-              if (last_kb && last_b) umma_commit_2sm(b_empty, 3);
-            } else {
-              umma_commit(&empty_bar[stage]);
-              if (last_kb) umma_commit(&tmem_full[acc]);
-              if (last_kb && last_b) umma_commit(b_empty);
-            }
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        first = false;
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-      if (dbg && lane == 0) {
-        g_gemm_dbg[0] = (unsigned long long)(clock64() - d_t0); g_gemm_dbg[1] = (unsigned long long)d_acc;
-        g_gemm_dbg[2] = (unsigned long long)d_full; g_gemm_dbg[3] = (unsigned long long)t_count;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      if (++kc == p.kc_per_tap) {
+        kc = 0;
+        if (++dx > p.taps_w - 1 - p.pad_w) { dx = -p.pad_w; ++dy; }
       }
     }
-  } else if (gemm_streaming(MODE) && warp == 10) {
-    // ===================== MODE 4: residual-load / output-store warp =====================
-    if (lane == 0) {
-      constexpr int NCH = BN / 32;
-      bool first = true;
-      int it = 0;
-      const bool dbg = kRoleTimers && dbgtime && blockIdx.x == 0;
-      long long d_c = 0, d_r = 0;
-      for (int ti = 0, tile = t_begin; ti < t_count; ++ti, tile += t_step, ++it) {
-        const int tcol = tile_col(tile);
-        int tm = tile_mu(tile) * NCTA + (int)cta_rank;
-        const int twi = tm % p.tiles_w; tm /= p.tiles_w;
-        const int thi = tm % p.tiles_h; tm /= p.tiles_h;
-        const int m0 = (tm * p.H + thi) * p.W + twi * p.tw;      // th == tn == 1: 128 consecutive output rows
-        const int n0 = tcol * BN;
-        if (first) {
-          for (int c = 0; c < NCH; ++c) {
-            if (p.has_res) {
-              mbar_arrive_expect_tx(&r_full[c], S::RCHUNK_BYTES);
-              tma_load_2d(staging + c * S::RCHUNK_BYTES, &p.mapRes, &r_full[c], n0 + c * 32, m0);
-            } else {
-              mbar_arrive(&r_full[c]);
-            }
-          }
-          first = false;
-        }
-        const int ntile = tile + t_step;
-        const bool has_next = ti + 1 < t_count;
-        int nm0 = 0, nn0 = 0;
-        if (has_next) {
-          int t2 = tile_mu(ntile) * NCTA + (int)cta_rank;
-          const int w2 = t2 % p.tiles_w; t2 /= p.tiles_w;
-          const int h2 = t2 % p.tiles_h; t2 /= p.tiles_h;
-          nm0 = (t2 * p.H + h2) * p.W + w2 * p.tw;
-          nn0 = tile_col(ntile) * BN;
-        }
-        // all chunk stores are issued back to back (one bulk group each); a chunk's buffer is only handed on once
-        // ITS group has been read out of shared memory — waiting per store serialised the store warp
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) {
-          { const long long w0 = dbg ? clock64() : 0; mbar_wait(&c_ready[c], (uint32_t)(it & 1)); if (dbg) d_c += clock64() - w0; }
-          if (dbgmode != 4) tma_store_2d(&p.mapOut, staging + c * S::RCHUNK_BYTES, n0 + c * 32, m0);
-          tma_store_commit();
-        }
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) {
-          { const long long w0 = dbg ? clock64() : 0; tma_store_wait_read_le(NCH - 1 - c); if (dbg) d_r += clock64() - w0; }   // groups complete in order
-          if (has_next) {
-            if (p.has_res) {
-              mbar_arrive_expect_tx(&r_full[c], S::RCHUNK_BYTES);
-              tma_load_2d(staging + c * S::RCHUNK_BYTES, &p.mapRes, &r_full[c], nn0 + c * 32, nm0);
-            } else {
-              mbar_arrive(&r_full[c]);
-            }
-          }
-        }
-      }
-      tma_store_wait_all();
-      if (dbg) { g_gemm_dbg[9] = (unsigned long long)d_c; g_gemm_dbg[10] = (unsigned long long)d_r; }
-    }
-  } else if (gemm_streaming(MODE)) {
-    // ===================== MODE 4/5: epilogue warps 2..9, thread == tile row =====================
-    const int ew = warp - 2;
-    const int lane_grp = warp & 3;
-    const int half = ew >> 2;
-    const int r = lane_grp * 32 + lane;
-    constexpr int NCH = BN / 32;
-    constexpr int MYCH = (NCH + 1) / 2;
-    const uint32_t te_addr0 = (NCTA == 2) ? mapa_shared(smem_u32(&tmem_empty[0]), 0) : smem_u32(&tmem_empty[0]);
-    int acc = 0, it = 0;
-    uint32_t acc_phase = 0;
-    const bool dbg = kRoleTimers && dbgtime && blockIdx.x == 0 && warp == 2;
-    long long d_t0 = dbg ? clock64() : 0, d_tf = 0, d_rf = 0;
-    for (int ti = 0, tile = t_begin; ti < t_count; ++ti, tile += t_step, ++it) {
-      const int tcol = tile_col(tile);
-      int tm = tile_mu(tile) * NCTA + (int)cta_rank;
-      const int twi = tm % p.tiles_w; tm /= p.tiles_w;
-      const int thi = tm % p.tiles_h; tm /= p.tiles_h;
-      const long long grow = (long long)(tm * p.H + thi) * p.W + twi * p.tw + r;
-      const int n_base = tcol * BN;
-      const bool row_ok = grow < (long long)p.NB * p.H * p.W;
-      float ln_mu = 0.f, ln_rstd = 1.f;
-      if (MODE == 8 && row_ok) {      // finish the LayerNorm statistics of this thread's row
-        float sm = 0.f, sq = 0.f;
-        const float2* st = reinterpret_cast<const float2*>(p.ln_stats_in) + grow * p.ln_parts_in;
-        for (int q = 0; q < p.ln_parts_in; ++q) { const float2 t2 = __ldg(st + q); sm += t2.x; sq += t2.y; }
-        ln_mu = sm * p.ln_inv_dim;
-        ln_rstd = rsqrtf(fmaxf(sq * p.ln_inv_dim - ln_mu * ln_mu, 0.f) + p.ln_eps);
-      }
-      f32x2 st_sum2 = 0ull, st_sq2 = 0ull;                        // partial row sums of what this thread stores (producer)
-      const uint32_t t_row = tmem_base + (uint32_t(lane_grp * 32) << 16) + acc * BN;
-#pragma unroll
-      for (int k = 0; k < MYCH; ++k) {
-        const int c = half + 2 * k;
-        if (c < NCH) {
-          // column vectors of this chunk (bias / folded-LayerNorm s_n): they do not depend on the accumulator, so they are
-          // requested BEFORE the wait for it — behind tcgen05.wait::ld their L2 round trip sat on the per-tile critical
-          // path of these latency-bound short-K tiles
-          const int n0 = n_base + c * 32;
-          float4 bq[8], sq4[8];
-          constexpr bool use_ln = MODE == 8;
-          if (p.bias != nullptr) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) bq[j] = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + 4 * j));
-          }
-          if (use_ln) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) sq4[j] = __ldg(reinterpret_cast<const float4*>(p.ln_colsum + n0 + 4 * j));
-          }
-          if (k == 0) {
-            { const long long w0 = dbg ? clock64() : 0; mbar_wait(&tmem_full[acc], acc_phase); if (dbg) d_tf += clock64() - w0; }
-            tc_fence_after();
-          }
-          uint32_t v[32];
-          tmem_ld_32x32(t_row + c * 32, v);
-          tmem_ld_wait();
-          if (c + 2 >= NCH) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if (NCTA == 2) mbar_arrive_cluster(te_addr0 + acc * 8);
-              else mbar_arrive(&tmem_empty[acc]);
-            }
-          }
-          float f[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-          if (use_ln) {
-            // out = rstd * acc + (-rstd * mean) * s_n + t_n : two packed FMAs per pair, bias (= t_n) included
-            const f32x2 a2 = f2_splat(ln_rstd), b2 = f2_splat(-ln_rstd * ln_mu);
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 s4 = sq4[j >> 2], t4 = bq[j >> 2];
-              f2_unpack(f2_fma(a2, f2_pack(f[j], f[j + 1]), f2_fma(b2, f2_pack(s4.x, s4.y), f2_pack(t4.x, t4.y))), f[j], f[j + 1]);
-              f2_unpack(f2_fma(a2, f2_pack(f[j + 2], f[j + 3]), f2_fma(b2, f2_pack(s4.z, s4.w), f2_pack(t4.z, t4.w))), f[j + 2], f[j + 3]);
-            }
-          } else if (p.bias != nullptr) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 b4 = bq[j >> 2];
-              f[j] += b4.x; f[j + 1] += b4.y; f[j + 2] += b4.z; f[j + 3] += b4.w;
-            }
-          }
-          if (p.rowvec != nullptr) {
-            const float* rv = p.rowvec + (long long)((grow / p.rows_per_group) % p.n_groups) * p.ldv;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 b4 = __ldg(reinterpret_cast<const float4*>(rv + n0 + j));
-              f[j] += b4.x; f[j + 1] += b4.y; f[j + 2] += b4.z; f[j + 3] += b4.w;
-            }
-          }
-          { const long long w0 = dbg ? clock64() : 0; mbar_wait(&r_full[c], (uint32_t)(it & 1)); if (dbg) d_rf += clock64() - w0; }
-          if ((dbgmode == 3 || dbgmode == 6 || dbgmode == 7)) {
-          } else if (gemm_stream_bf16(MODE)) {
-            // 32 bf16 = 64 B per row; TMA SWIZZLE_64B: 16-byte chunk index ^= (row >> 1) & 3
-            uint8_t* rowp = staging + c * S::RCHUNK_BYTES + r * 64;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              uint4* q = reinterpret_cast<uint4*>(rowp + ((j ^ ((r >> 1) & 3)) << 4));
-              if (p.has_res) {     // bf16 residual tile (TMA-loaded into this chunk): add in fp32, round once
-                const uint4 a = *q;
-                const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&a);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 t = __bfloat1622float2(h[e]);
-                  f[8 * j + 2 * e] += t.x; f[8 * j + 2 * e + 1] += t.y;
-                }
-              }
-              const uint4 o4 = make_uint4(pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
-                                          pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
-              *q = o4;
-              if (MODE == 7) {                           // row sums of the fp32 values (their bf16 rounding, which the
-#pragma unroll                                           // consumer's MMA reads, perturbs mean / variance by < 2^-9 / sqrt(C))
-                for (int e = 0; e < 8; e += 2) {
-                  const f32x2 pr = f2_pack(f[8 * j + e], f[8 * j + e + 1]);
-                  st_sum2 = f2_add(st_sum2, pr);
-                  st_sq2 = f2_fma(pr, pr, st_sq2);
-                }
-              }
-            }
-          } else {
-            uint8_t* rowp = staging + c * S::RCHUNK_BYTES + r * 128;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4* q = reinterpret_cast<float4*>(rowp + ((j ^ (r & 7)) << 4));
-              float4 o = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-              if (p.has_res) {
-                const float4 a = *q;
-                o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
-              }
-              *q = o;
-            }
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&c_ready[c]);
-        }
-      }
-      if (MODE == 7 && row_ok) {
-        float s0, s1, q0, q1;
-        f2_unpack(st_sum2, s0, s1);
-        f2_unpack(st_sq2, q0, q1);
-        reinterpret_cast<float2*>(p.ln_stats_out)[grow * p.ln_parts_out + tcol * 2 + half] = make_float2(s0 + s1, q0 + q1);
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-    if (dbg && lane == 0) {
-      g_gemm_dbg[6] = (unsigned long long)(clock64() - d_t0); g_gemm_dbg[7] = (unsigned long long)d_tf; g_gemm_dbg[8] = (unsigned long long)d_rf;
-    }
-  } else {
-    // ===================== epilogue warps: TMEM lane quarter = warp & 3, chunk residue = (warp - 2) / 4 ==========
-    // EG warps share a lane quarter and split the 32-column chunks between them (c mod EG). Everything a warp
-    // needs from global memory for its chunks (the fp32 residual) is requested at tile start, before the accumulator
-    // is even ready, so the DRAM round trip overlaps the main loop instead of serialising the epilogue.
-    const int ew = warp - 2;
-    const int lane_grp = warp & 3;
-    const int half = ew >> 2;                    // chunk residue class of this warp
-    uint8_t* my_stage = staging + ew * S::STAGE_WARP_BYTES;
-    int* my_rowmap = rowmap + ew * 32;
-    float* my_bias = reinterpret_cast<float*>(rowmap + NEPI * 32) + ew * 128;   // bias of this warp's <= 4 chunks
-    constexpr int NCH = BN / 32;
-    constexpr int MYCH = (NCH + EG - 1) / EG;
-    constexpr int PRECH = MYCH < 2 ? MYCH : 2;   // chunks whose residual is prefetched at tile start (register budget:
-                                                 // a third chunk spills, and a spilled prefetch stalls on its own load)
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    int bias_col = -1;                           // column tile whose bias slice sits in my_bias
-    // hand-back target: the leader CTA's tmem_empty barrier (remote arrive from the peer CTA of a pair)
-    const uint32_t te_addr0 = (NCTA == 2) ? mapa_shared(smem_u32(&tmem_empty[0]), 0) : smem_u32(&tmem_empty[0]);
-    auto release_acc = [&](int a) {
-      if (NCTA == 2) mbar_arrive_cluster(te_addr0 + a * 8);
-      else mbar_arrive(&tmem_empty[a]);
-    };
-    for (int ti = 0, tile = t_begin; ti < t_count; ++ti, tile += t_step) {
-      const int tcol = tile_col(tile);
-      int tm = tile_mu(tile) * NCTA + (int)cta_rank;
-      const int twi = tm % p.tiles_w; tm /= p.tiles_w;
-      const int thi = tm % p.tiles_h; tm /= p.tiles_h;
-      const int tni = tm;
-      // output row of the tile row this thread owns (tile rows are ordered [tn][th][tw] = TMA box order)
-      {
-        const int r = lane_grp * 32 + lane;
-        const int dx = r % p.tw;
-        const int dy = (r / p.tw) % p.th;
-        const int dn = r / (p.tw * p.th);
-        const int x = twi * p.tw + dx, y = thi * p.th + dy, n = tni * p.tn + dn;
-        const bool ok = (x < p.W) && (y < p.H) && (n < p.NB);
-        my_rowmap[lane] = ok ? ((n * p.H + y) * p.W + x) : -1;
-      }
-      const int n_base = tcol * BN;
-      // bias slice of this warp's chunks -> shared memory now, while the accumulator is still being computed (a global
-      // load per chunk inside the epilogue left the warps on the long scoreboard for a third of their time)
-      if (S::BIAS_SMEM && p.bias != nullptr && tcol != bias_col) {     // (the weight-stationary schedule keeps one column tile)
-#pragma unroll
-        for (int k = 0; k < MYCH; ++k) {
-          const int n = n_base + (half + EG * k) * 32 + lane;
-          my_bias[k * 32 + lane] = (half + EG * k < NCH && n < p.N) ? __ldg(p.bias + n) : 0.f;
-        }
-        bias_col = tcol;
-      }
-      __syncwarp();
-      const int my_row = my_rowmap[lane];
-      // ---- residual prefetch (fp32 output path): lane -> (row i*4 + lane/8, 16-byte column chunk lane%8)
-      float4 rpre[PRECH][8];
-      const bool pre = (MODE == 0 || MODE == 3) && (p.residual != nullptr);
-      if (pre) {
-#pragma unroll
-        for (int k = 0; k < PRECH; ++k) {
-          const int c = half + EG * k;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int grow = my_rowmap[i * 4 + (lane >> 3)];
-            const int col = n_base + c * 32 + (lane & 7) * 4;
-            rpre[k][i] = (c < NCH && grow >= 0 && col < p.N)
-                             ? *reinterpret_cast<const float4*>(p.residual + (long long)grow * p.ldr + col)
-                             : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-        }
-      }
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      if (half >= NCH) {   // narrow tiles: warps that own no chunk still take part in the hand-back
-        __syncwarp();
-        if (lane == 0) release_acc(acc);
-      }
-      const uint32_t t_row = tmem_base + (uint32_t(lane_grp * 32) << 16) + acc * BN;
-#pragma unroll
-      for (int k = 0; k < MYCH; ++k) {
-        const int c = half + EG * k;
-        if (c < NCH) {
-          uint32_t v[32];
-          tmem_ld_32x32(t_row + c * 32, v);
-          tmem_ld_wait();
-          if (c + EG >= NCH) {
-            // last TMEM read of this warp for this accumulator stage -> hand it back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) release_acc(acc);
-          }
-          if ((dbgmode == 3 || dbgmode == 6 || dbgmode == 7)) continue;
-          const int n0 = n_base + c * 32;
-          float f[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-          if (p.bias != nullptr) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (S::BIAS_SMEM) b4 = *reinterpret_cast<const float4*>(my_bias + k * 32 + j);   // broadcast read; 0 beyond N
-              else if (n0 + j < p.N) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + j));
-              f2_unpack(f2_add(f2_pack(f[j], f[j + 1]), f2_pack(b4.x, b4.y)), f[j], f[j + 1]);
-              f2_unpack(f2_add(f2_pack(f[j + 2], f[j + 3]), f2_pack(b4.z, b4.w)), f[j + 2], f[j + 3]);
-            }
-          }
-          if (p.rowvec != nullptr && my_row >= 0) {
-            const float* rv = p.rowvec + (long long)((my_row / p.rows_per_group) % p.n_groups) * p.ldv;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              if (n0 + j < p.N) {
-                const float4 b4 = __ldg(reinterpret_cast<const float4*>(rv + n0 + j));
-                f2_unpack(f2_add(f2_pack(f[j], f[j + 1]), f2_pack(b4.x, b4.y)), f[j], f[j + 1]);
-                f2_unpack(f2_add(f2_pack(f[j + 2], f[j + 3]), f2_pack(b4.z, b4.w)), f[j + 2], f[j + 3]);
-              }
-            }
-          }
-          if (MODE == 2) {
-            // chunk = 16 value columns then the 16 gate columns of the same outputs: out = value * gelu_erf(gate)
-            // (reference GEGLU: attention.py:97-99, exact erf GELU); two outputs per packed fp32x2 instruction
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const f32x2 o = geglu_f32x2(f2_pack(f[2 * j], f[2 * j + 1]), f2_pack(f[16 + 2 * j], f[16 + 2 * j + 1]));
-              f2_unpack(o, f[2 * j], f[2 * j + 1]);
-            }
-            uint4* dst = reinterpret_cast<uint4*>(my_stage + lane * 32);   // 16 bf16 = 32 B per row
-            dst[0] = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
-            dst[1] = make_uint4(pack_bf16x2(f[8], f[9]), pack_bf16x2(f[10], f[11]), pack_bf16x2(f[12], f[13]), pack_bf16x2(f[14], f[15]));
-            __syncwarp();
-            __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
-            const int no0 = n0 / 2;
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              const int rr = i * 16 + (lane >> 1);
-              const int ch = lane & 1;
-              const int grow = my_rowmap[rr];
-              if (grow >= 0 && no0 + ch * 8 < p.N / 2 && dbgmode != 4) {
-                const uint4 val = *reinterpret_cast<const uint4*>(my_stage + rr * 32 + ch * 16);
-                *reinterpret_cast<uint4*>(out + (long long)grow * p.ldo + no0 + ch * 8) = val;
-              }
-            }
-          } else if (MODE == 1) {
-            // 32 bf16 = 64 B per row, 16 B chunks XOR-swizzled with (row>>1)&3
-#pragma unroll
-            for (int ch = 0; ch < 4; ++ch) {
-              const int sw = ch ^ ((lane >> 1) & 3);
-              *reinterpret_cast<uint4*>(my_stage + lane * 64 + sw * 16) =
-                  make_uint4(pack_bf16x2(f[ch * 8 + 0], f[ch * 8 + 1]), pack_bf16x2(f[ch * 8 + 2], f[ch * 8 + 3]),
-                             pack_bf16x2(f[ch * 8 + 4], f[ch * 8 + 5]), pack_bf16x2(f[ch * 8 + 6], f[ch * 8 + 7]));
-            }
-            __syncwarp();
-            __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int rr = i * 8 + (lane >> 2);
-              const int ch = lane & 3;
-              const int grow = my_rowmap[rr];
-              if (grow >= 0 && n0 + ch * 8 < p.N && dbgmode != 4) {
-                const int sw = ch ^ ((rr >> 1) & 3);
-                uint4 val = *reinterpret_cast<const uint4*>(my_stage + rr * 64 + sw * 16);
-                if (p.residual != nullptr) {
-                  float4 r0, r1;
-                  if (p.res_bf16) {
-                    const uint4 rb = *reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.residual) +
-                                                                     (long long)grow * p.ldr + n0 + ch * 8);
-                    const __nv_bfloat162* hb = reinterpret_cast<const __nv_bfloat162*>(&rb);
-                    const float2 t0 = __bfloat1622float2(hb[0]), t1 = __bfloat1622float2(hb[1]);
-                    const float2 t2 = __bfloat1622float2(hb[2]), t3 = __bfloat1622float2(hb[3]);
-                    r0 = make_float4(t0.x, t0.y, t1.x, t1.y); r1 = make_float4(t2.x, t2.y, t3.x, t3.y);
-                  } else {
-                    const float* rp = p.residual + (long long)grow * p.ldr + n0 + ch * 8;
-                    r0 = *reinterpret_cast<const float4*>(rp);
-                    r1 = *reinterpret_cast<const float4*>(rp + 4);
-                  }
-                  __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&val);
-                  float2 a = __bfloat1622float2(h[0]), b = __bfloat1622float2(h[1]);
-                  float2 c2 = __bfloat1622float2(h[2]), d = __bfloat1622float2(h[3]);
-                  val = make_uint4(pack_bf16x2(a.x + r0.x, a.y + r0.y), pack_bf16x2(b.x + r0.z, b.y + r0.w),
-                                   pack_bf16x2(c2.x + r1.x, c2.y + r1.y), pack_bf16x2(d.x + r1.z, d.y + r1.w));
-                }
-                *reinterpret_cast<uint4*>(out + (long long)grow * p.ldo + n0 + ch * 8) = val;
-              }
-            }
-          } else {
-            // 32 fp32 = 128 B per row, 16 B chunks XOR-swizzled with row&7 (conflict-free both ways)
-#pragma unroll
-            for (int ch = 0; ch < 8; ++ch) {
-              const int sw = ch ^ (lane & 7);
-              *reinterpret_cast<float4*>(my_stage + lane * 128 + sw * 16) =
-                  make_float4(f[ch * 4 + 0], f[ch * 4 + 1], f[ch * 4 + 2], f[ch * 4 + 3]);
-            }
-            __syncwarp();
-            float* out = reinterpret_cast<float*>(p.out);
-            const int ch = lane & 7;
-            const bool col_ok = n0 + ch * 4 < p.N;
-            float4 r2[8];
-            if (MODE == 3) {
-              // second addend: all eight loads are issued before the first store (out may alias a residual)
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const int grow = my_rowmap[i * 4 + (lane >> 3)];
-                r2[i] = (grow >= 0 && col_ok)
-                            ? *reinterpret_cast<const float4*>(p.residual2 + (long long)grow * p.ldr2 + n0 + ch * 4)
-                            : make_float4(0.f, 0.f, 0.f, 0.f);
-              }
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int rr = i * 4 + (lane >> 3);
-              const int grow = my_rowmap[rr];
-              if (grow >= 0 && col_ok && dbgmode != 4) {
-                const int sw = ch ^ (rr & 7);
-                float4 val = *reinterpret_cast<const float4*>(my_stage + rr * 128 + sw * 16);
-                if (pre) {
-                  float4 rr4;
-                  if (k < PRECH) rr4 = rpre[k < PRECH ? k : 0][i];
-                  else rr4 = *reinterpret_cast<const float4*>(p.residual + (long long)grow * p.ldr + n0 + ch * 4);
-                  val.x += rr4.x; val.y += rr4.y; val.z += rr4.z; val.w += rr4.w;
-                }
-                if (MODE == 3) { val.x += r2[i].x; val.y += r2[i].y; val.z += r2[i].z; val.w += r2[i].w; }
-                *reinterpret_cast<float4*>(out + (long long)grow * p.ldo + n0 + ch * 4) = val;
-              }
-            }
-          }
-        }
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
+    return;
   }
 
-  tc_fence_before();
-  if (NCTA == 2) cluster_sync_all();   // the leader's MMAs read the peer's smem/TMEM: nobody leaves early
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if (NCTA == 2) tmem_dealloc_2sm(tmem_base, TMEM_COLS);
-    else tmem_dealloc(tmem_base, TMEM_COLS);
+  // ===================== consumer warpgroups =====================
+  const int wg = warp >> 2;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  {
+    const uint32_t base = smem_u32(smem);
+    const uint64_t descA0 = wgmma_desc(base + wg * (64 * 128), 16, 1024, kSw128);
+    const uint64_t descB0 = wgmma_desc(base + S::A_BYTES, 16, 1024, kSw128);
+    constexpr uint64_t STAGE_STEP = S::STAGE_BYTES >> 4;      // start-address field is in 16-byte units
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < num_k_blocks; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+        wgmma_ss<BN>(acc, descA0 + STAGE_STEP * stage + 2 * k, descB0 + STAGE_STEP * stage + 2 * k, (kb > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();                         // the group of the previous k-block has retired: refill its stage
+      if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+  }
+
+  // ===================== epilogue: this thread owns tile rows r0 and r0 + 8, columns 8j + 2 (lane % 4) + {0, 1} =====
+  const int quad = lane & 3;
+  long long grow[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // tile rows are ordered [tn][th][tw] = TMA box order
+    const int x = twi * p.tw + r % p.tw, y = thi * p.th + (r / p.tw) % p.th, n = tni * p.tn + r / (p.tw * p.th);
+    grow[h] = (x < p.W && y < p.H && n < p.NB) ? ((long long)n * p.H + y) * p.W + x : -1;
+  }
+  const int n_base = tcol * BN + 2 * quad;
+
+  if (MODE == 2) {
+    // chunk of 32 columns = 16 value columns then the 16 gate columns of the same outputs: out = value * gelu_erf(gate)
+    // (reference GEGLU: attention.py:97-99, exact erf GELU). Block j (j % 4 < 2) holds values, block j + 2 their gates.
+    __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      if ((j & 3) >= 2) continue;
+      const int n = n_base + 8 * j;
+      if (n >= p.N) continue;
+      const float2 bv = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
+      const float2 bg = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n + 16)) : make_float2(0.f, 0.f);
+      const int no = (tcol * BN) / 2 + (j >> 2) * 16 + (j & 1) * 8 + 2 * quad;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (grow[h] < 0) continue;
+        float v0 = acc[4 * j + 2 * h] + bv.x, v1 = acc[4 * j + 2 * h + 1] + bv.y;
+        float g0 = acc[4 * (j + 2) + 2 * h] + bg.x, g1 = acc[4 * (j + 2) + 2 * h + 1] + bg.y;
+        if (p.rowvec != nullptr) {
+          const float* rv = p.rowvec + (long long)((grow[h] / p.rows_per_group) % p.n_groups) * p.ldv;
+          v0 += rv[n]; v1 += rv[n + 1]; g0 += rv[n + 16]; g1 += rv[n + 17];
+        }
+        *reinterpret_cast<uint32_t*>(out + grow[h] * p.ldo + no) = pack_bf16x2(geglu_f32(v0, g0), geglu_f32(v1, g1));
+      }
+    }
+    return;
+  }
+
+  float ln_a[2] = {1.f, 1.f}, ln_b[2] = {0.f, 0.f};       // folded LayerNorm: out = a * acc + b * s_n + t_n
+  if (MODE == 1 && p.ln_stats_in != nullptr) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (grow[h] < 0) continue;
+      float sm = 0.f, sq = 0.f;
+      const float2* st = reinterpret_cast<const float2*>(p.ln_stats_in) + grow[h] * p.ln_parts_in;
+      for (int q = 0; q < p.ln_parts_in; ++q) { const float2 t2 = __ldg(st + q); sm += t2.x; sq += t2.y; }
+      const float mu = sm * p.ln_inv_dim;
+      const float rstd = rsqrtf(fmaxf(sq * p.ln_inv_dim - mu * mu, 0.f) + p.ln_eps);
+      ln_a[h] = rstd;
+      ln_b[h] = -rstd * mu;
+    }
+  }
+  float st_sum[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, st_sq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][column half]
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int n = n_base + 8 * j;
+    if (n >= p.N) continue;
+    const float2 b2 = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
+    float2 s2 = make_float2(0.f, 0.f);
+    if (MODE == 1 && p.ln_stats_in != nullptr) s2 = __ldg(reinterpret_cast<const float2*>(p.ln_colsum + n));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (grow[h] < 0) continue;
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      if (MODE == 1 && p.ln_stats_in != nullptr) {
+        v0 = fmaf(ln_a[h], v0, fmaf(ln_b[h], s2.x, b2.x));
+        v1 = fmaf(ln_a[h], v1, fmaf(ln_b[h], s2.y, b2.y));
+      } else {
+        v0 += b2.x; v1 += b2.y;
+      }
+      if (p.rowvec != nullptr) {
+        const float2 r2 = __ldg(reinterpret_cast<const float2*>(
+            p.rowvec + (long long)((grow[h] / p.rows_per_group) % p.n_groups) * p.ldv + n));
+        v0 += r2.x; v1 += r2.y;
+      }
+      if (p.residual != nullptr) {
+        if (MODE == 1 && p.res_bf16) {
+          const float2 r2 = __bfloat1622float2(
+              *reinterpret_cast<const __nv_bfloat162*>(reinterpret_cast<const __nv_bfloat16*>(p.residual) + grow[h] * p.ldr + n));
+          v0 += r2.x; v1 += r2.y;
+        } else {
+          const float2 r2 = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.residual) + grow[h] * p.ldr + n);
+          v0 += r2.x; v1 += r2.y;
+        }
+      }
+      if (MODE == 0) {
+        if (p.residual2 != nullptr) {
+          const float2 r2 = *reinterpret_cast<const float2*>(p.residual2 + grow[h] * p.ldr2 + n);
+          v0 += r2.x; v1 += r2.y;
+        }
+        *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + grow[h] * p.ldo + n) = make_float2(v0, v1);
+      } else {
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + grow[h] * p.ldo + n) = pack_bf16x2(v0, v1);
+        // row sums of the fp32 values (their bf16 rounding, which the consumer's MMA reads, perturbs mean / variance
+        // by < 2^-9 / sqrt(C))
+        const int hf = j < NJ / 2 ? 0 : 1;
+        st_sum[h][hf] += v0 + v1;
+        st_sq[h][hf] = fmaf(v0, v0, fmaf(v1, v1, st_sq[h][hf]));
+      }
+    }
+  }
+  if (MODE == 1 && p.ln_stats_out != nullptr) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        float s = st_sum[h][hf], q = st_sq[h][hf];
+        s += __shfl_xor_sync(0xffffffffu, s, 1); s += __shfl_xor_sync(0xffffffffu, s, 2);
+        q += __shfl_xor_sync(0xffffffffu, q, 1); q += __shfl_xor_sync(0xffffffffu, q, 2);
+        if (quad == 0 && grow[h] >= 0)
+          reinterpret_cast<float2*>(p.ln_stats_out)[grow[h] * p.ln_parts_out + tcol * 2 + hf] = make_float2(s, q);
+      }
+    }
   }
 }
 
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static int gemm_stream_kmax() {
-  static int kmax = -1;
-  if (kmax < 0) {
-    const char* e = getenv("PN_GEMM_STREAM_KMAX");     // 0 disables the streaming epilogue
-    kmax = e ? atoi(e) : 1920;
-  }
-  return kmax;
-}
-
-static int gemm_bstat_enabled() {   // PN_GEMM_BSTAT=0 disables the weight-stationary schedule (A/B measurements)
-  static int m = -1;
-  if (m < 0) {
-    const char* e = getenv("PN_GEMM_BSTAT");
-    m = e ? atoi(e) : 1;
-  }
-  return m;
-}
-
-static int gemm_force_bn() {      // PN_GEMM_BN: force the N tile of the non-streaming CTA-pair path (experiments)
-  static int m = -1;
-  if (m < 0) {
-    const char* e = getenv("PN_GEMM_BN");
-    m = e ? atoi(e) : 0;
-  }
-  return m;
-}
-
-#ifdef PN_GEMM_ROLE_TIMERS
-static int gemm_debug_mode() {
-  static int m = -1;
-  if (m < 0) {
-    const char* e = getenv("PN_GEMM_DEBUG");
-    m = e ? atoi(e) : 0;
-  }
-  return m;
-}
-#endif
-
-static int conv_halo_mode() {     // PN_CONV_HALO=0 disables the haloed 3x3 conv (A/B measurements); the row-shifted A views use
-                                   // descriptor base_offset 0 (verified on B200: the 128B swizzle is a function of the absolute
-                                   // shared-memory address)
-  static int m = -1;
-  if (m < 0) {
-    const char* e = getenv("PN_CONV_HALO");
-    m = e ? atoi(e) : 2;
-  }
-  return m;
-}
-
-static int gemm_mode_override() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("PN_GEMM_MODE");
-    mode = e ? atoi(e) : 0;
-  }
-  return mode;
-}
-
 // Pick the [tn, th, tw] box (product 128, powers of two) that wastes the fewest MMA rows.
 static void pick_tile(long long NB, long long H, long long W, int* tw, int* th, int* tn) {
   double best = 1e30;
@@ -978,30 +284,16 @@ static void pick_tile(long long NB, long long H, long long W, int* tw, int* th, 
   }
 }
 
-template <int BN, int STAGES, int NCTA, int MODE>
-static int launch_gemm_mode(const GemmParams& p, cudaStream_t stream) {
-  using S = GemmSmem<BN, STAGES, NCTA, MODE>;
-  static_assert(S::TOTAL <= 232448, "shared memory budget exceeded");
-  {
-    const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(&gemm_tc_kernel<BN, STAGES, NCTA, MODE>), S::TOTAL);
-    if (rc != PN_OK) return rc;
-  }
-  const int tiles_m = p.tiles_w * p.tiles_h * p.tiles_n;
-  const int num_tiles = ((tiles_m + NCTA - 1) / NCTA) * p.tiles_col;
-  int units = sm_count() / NCTA;
-  if (units > num_tiles) units = num_tiles;
-  PN_CHECK_CUDA(launch_kernel(gemm_tc_kernel<BN, STAGES, NCTA, MODE>, dim3(units * NCTA), dim3(gemm_threads(MODE)), S::TOTAL, stream,
-                             NCTA, p));
+template <int BN, int STAGES>
+static int launch_gemm(const GemmParams& p, int mode, long long tiles, cudaStream_t stream) {
+  using S = GemmSmem<BN, STAGES>;
+  static_assert(S::TOTAL <= 232448, "shared memory budget exceeded (227 KB per block)");
+  void (*kern)(GemmParams) = mode == 2 ? gemm_tc_kernel<BN, STAGES, 2> : mode == 1 ? gemm_tc_kernel<BN, STAGES, 1>
+                                                                                   : gemm_tc_kernel<BN, STAGES, 0>;
+  const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), S::TOTAL);
+  if (rc != PN_OK) return rc;
+  PN_CHECK_CUDA(launch_kernel(kern, dim3((unsigned)tiles), dim3(GEMM_THREADS), S::TOTAL, stream, 1, p));
   return PN_OK;
-}
-
-template <int BN, int STAGES, int NCTA>
-static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
-  // GEGLU runs 16 epilogue warps (its epilogue, not the k loop, is the long pole): one ring stage pays for their staging
-  if (p.geglu) return launch_gemm_mode<BN, (STAGES > 4 ? STAGES - 1 : STAGES), NCTA, 2>(p, stream);
-  if (p.out_bf16) return launch_gemm_mode<BN, STAGES, NCTA, 1>(p, stream);
-  if (p.residual2 != nullptr) return launch_gemm_mode<BN, STAGES, NCTA, 3>(p, stream);
-  return launch_gemm_mode<BN, STAGES, NCTA, 0>(p, stream);
 }
 
 }  // namespace pn
@@ -1032,6 +324,7 @@ extern "C" int pn_gemm(const pn_gemm_args* a, void* stream_v) {
   if (a->ln_stats_in) PN_REQUIRE(a->ln_colsum && a->ln_parts_in > 0 && a->ln_parts_in <= 64 && a->out_bf16 && !a->geglu && a->taps_h == 1 && a->taps_w == 1,
                                  "pn_gemm: a folded LayerNorm needs ln_colsum, 1..64 partial sums per row, a 1x1 GEMM and bf16 output");
 
+
   GemmParams p;
   std::memset(&p, 0, sizeof(p));
   long long NB = a->NB, H = a->H, W = a->W;
@@ -1051,145 +344,51 @@ extern "C" int pn_gemm(const pn_gemm_args* a, void* stream_v) {
   p.taps_h = a->taps_h; p.taps_w = a->taps_w;
   p.pad_h = a->taps_h / 2; p.pad_w = a->taps_w / 2;
   p.N = a->N;
-  p.out = a->out; p.bias = a->bias; p.rowvec = a->rowvec; p.residual = reinterpret_cast<const float*>(a->residual);
+  p.out = a->out; p.bias = a->bias; p.rowvec = a->rowvec; p.residual = a->residual;
   p.residual2 = a->residual2;
-#ifdef PN_GEMM_ROLE_TIMERS
-  p.debug = gemm_debug_mode();
-#endif
   p.ldo = a->ldo; p.ldr = a->ldr; p.ldr2 = a->ldr2;
   p.ldv = a->rowvec_ld > 0 ? a->rowvec_ld : a->N;
   p.rows_per_group = a->rows_per_group > 0 ? a->rows_per_group : 1;
   p.n_groups = a->n_groups > 0 ? a->n_groups : 1;
-  p.out_bf16 = a->out_bf16; p.geglu = a->geglu; p.res_bf16 = a->residual_bf16;
+  p.res_bf16 = a->residual_bf16;
   p.ln_stats_in = a->ln_stats_in; p.ln_colsum = a->ln_colsum; p.ln_stats_out = a->ln_stats_out;
   p.ln_parts_in = a->ln_parts_in; p.ln_eps = a->ln_eps; p.ln_inv_dim = 1.0f / (float)a->C;
 
-  // Tile selection. Big problems run on CTA pairs (cta_group::2, 256 x BN tiles: the weight tile is fetched once per
-  // pair, which is what lifts the L2->SM-bound K loop); small ones keep single-CTA 128 x BN tiles for parallelism.
-  // Every channel count of the network is a multiple of 160 (320/640/960/1280/1920/2560/5120/10240).
-  const long long tiles_m_1 = (long long)p.tiles_w * p.tiles_h * p.tiles_n;
-  int BN, NCTA = 1;
-  const int force = gemm_mode_override();     // PN_GEMM_MODE=1|2 (debug / A-B measurements)
-  // (a single-CTA 128 x N tile is L2->SM bound — 10.9 TB/s of operand traffic at 0.8 PF on the level-3 convs —, so pairs win
-  // as soon as they keep half of the SMs busy: 99 -> 68 us and 188 -> 118 us for the 1280- and 2560-channel 3x3 convs on
-  // 2,688 rows, tools/smallm_probe.py; they used to need two full waves of tiles)
-  const long long pair_min = sm_count() / 2;
-  if (a->N % 256 == 0 && (force == 2 || (force == 0 && tiles_m_1 * (a->N / 256) >= pair_min))) { BN = 256; NCTA = 2; }
-  else if (a->N % 160 == 0 && (force == 2 || (force == 0 && tiles_m_1 * (a->N / 160) >= pair_min))) { BN = 160; NCTA = 2; }
-  else if (a->N % 160 == 0) BN = 160;
-  else if (a->N >= 128) BN = 128;
-  else if (a->N > 32) BN = 64;
-  else BN = 32;
-  if (gemm_force_bn() > 0 && a->N % 32 == 0) { BN = gemm_force_bn(); NCTA = 2; }
-  // Haloed 3x3 conv (MODE 6): 16 x 8-pixel tiles, level-0/1 shapes whose N tile is 160 wide (L2->SM-bound otherwise).
-  bool halo_mode = conv_halo_mode() != 0 && a->taps_h == 3 && a->taps_w == 3 && !a->out_bf16 && !a->geglu &&
-                   a->residual == nullptr && a->residual2 == nullptr && a->N % 160 == 0 && a->N % 256 != 0 && H % 16 == 0 &&
-                   W % 8 == 0 && force != 1;
-  if (halo_mode) {
-    tw = 8; th = 16; tn = 1;
-    p.tw = tw; p.th = th; p.tn = tn;
-    p.tiles_w = (int)(W / 8); p.tiles_h = (int)(H / 16); p.tiles_n = (int)NB;
-    BN = 160;
-    const long long tiles_m_h = (long long)p.tiles_w * p.tiles_h * p.tiles_n;
-    NCTA = (tiles_m_h * (a->N / 160) >= 2 * sm_count() || force == 2) ? 2 : 1;
-  }
-  // Streaming epilogue (MODE 4): fp32 output whose tile rows are consecutive output rows, short K loop (HBM-bound).
-  const long long k_total = (long long)a->taps_h * a->taps_w * a->C;
-  const bool rows_contig = (tw == 128 && th == 1 && tn == 1) && ((H == 1 && NB == 1) || (W % 128 == 0));
-  const bool stream_bf16 = a->out_bf16 && !a->geglu && (a->residual == nullptr || a->residual_bf16) && a->ldo % 8 == 0;
-  const bool stream_f32 = !a->out_bf16 && !a->geglu && a->ldo % 4 == 0 && (a->residual == nullptr || a->ldr % 4 == 0);
-  // measured on B200: the fp32 variant wins up to K = 1920 (ff2 at level 0, temporal conv), the bf16 variant up to K = 640
-  const long long kmax = stream_bf16 ? (gemm_stream_kmax() < 640 ? gemm_stream_kmax() : 640) : gemm_stream_kmax();
-  bool stream_mode = (stream_bf16 || stream_f32) && a->residual2 == nullptr && rows_contig && k_total <= kmax &&
-                     (a->N % 160 == 0 || a->N % 128 == 0);
-  if (stream_mode) {
-    BN = (a->N % 160 == 0) ? 160 : 128;
-    NCTA = (force == 2 || (force == 0 && tiles_m_1 * (a->N / BN) >= 2 * sm_count())) ? 2 : 1;
-    const uint64_t rows_total = (uint64_t)NB * H * W;
-    int rc2;
-    if (stream_bf16) {
-      const uint64_t dimsO[2] = {(uint64_t)a->N, rows_total};
-      const uint64_t strO[1] = {(uint64_t)a->ldo};
-      const uint32_t boxO[2] = {32u, 128u};
-      rc2 = cached_tmap_bf16(&p.mapOut, a->out, 2, dimsO, strO, boxO, 64);
-    } else {
-      rc2 = cached_tmap_f32_2d(&p.mapOut, a->out, (uint64_t)a->N, rows_total, (uint64_t)a->ldo, 128u);
-    }
-    if (rc2 != PN_OK) return rc2;
-    p.has_res = a->residual != nullptr ? 1 : 0;
-    if (p.has_res) {
-      if (stream_bf16) {
-        const uint64_t dimsR[2] = {(uint64_t)a->N, rows_total};
-        const uint64_t strR[1] = {(uint64_t)a->ldr};
-        const uint32_t boxR[2] = {32u, 128u};
-        rc2 = cached_tmap_bf16(&p.mapRes, a->residual, 2, dimsR, strR, boxR, 64);
-      } else {
-        rc2 = cached_tmap_f32_2d(&p.mapRes, a->residual, (uint64_t)a->N, rows_total, (uint64_t)a->ldr, 128u);
-      }
-      if (rc2 != PN_OK) return rc2;
-    }
-  }
+  // N tile: every channel count of the network is a multiple of 160 (320/640/960/1280/1920/2560/5120/10240); a
+  // 128 x 160 fp32 accumulator is 80 registers per consumer thread.
+  const int BN = a->N % 160 == 0 ? 160 : a->N >= 128 ? 128 : a->N > 32 ? 64 : 32;
   p.tiles_col = (a->N + BN - 1) / BN;
   if (a->ln_stats_out) {
-    PN_REQUIRE(stream_mode && a->out_bf16, "pn_gemm: ln_stats_out needs the streaming bf16 epilogue (1x1 GEMM, K <= 640, bf16 out, N %% 160 or 128 == 0)");
+    PN_REQUIRE(a->out_bf16 && !a->geglu && a->ln_stats_in == nullptr && pn_gemm_ln_parts(a->N) == 2 * p.tiles_col,
+               "pn_gemm: ln_stats_out needs bf16 out, no GEGLU, no folded LayerNorm input and N %% 160 or 128 == 0");
     p.ln_parts_out = 2 * p.tiles_col;
   }
-  if (a->ln_stats_in) PN_REQUIRE(stream_mode && a->out_bf16 && a->ln_stats_out == nullptr,
-                                 "pn_gemm: a folded LayerNorm needs the streaming bf16 epilogue (1x1 GEMM, K <= 640) and cannot also emit row sums");
-  // weight-stationary schedule: 1x1 GEMMs with K = 320 (5 k-blocks, every ring has >= 5 stages) and enough column
-  // tiles and row tiles for the saved weight traffic to matter
-  p.bstat = (gemm_bstat_enabled() && !halo_mode && a->taps_h == 1 && a->taps_w == 1 && a->C == 5 * BK && p.tiles_col >= 3 &&
-             NCTA == 2 && tiles_m_1 >= 8 * sm_count() && p.tiles_col <= sm_count() / 8) ? 1 : 0;
+  const long long tiles = (long long)p.tiles_w * p.tiles_h * p.tiles_n * p.tiles_col;
+  PN_REQUIRE(tiles > 0 && tiles < (1ll << 31), "pn_gemm: too many output tiles");
 
   const uint64_t dimsA[4] = {(uint64_t)a->C, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
   const uint64_t strA[3] = {(uint64_t)sw, (uint64_t)sh, (uint64_t)sn};
-  const uint32_t boxA[4] = {64u, (uint32_t)(halo_mode ? tw + 2 : tw), (uint32_t)(halo_mode ? th + 2 : th), (uint32_t)tn};
+  const uint32_t boxA[4] = {64u, (uint32_t)tw, (uint32_t)th, (uint32_t)tn};
   int rc = cached_tmap_bf16(&p.mapA, a->A, 4, dimsA, strA, boxA, 128);
   if (rc != PN_OK) return rc;
   const uint64_t K = (uint64_t)a->taps_h * a->taps_w * a->C;
   const uint64_t dimsB[2] = {K, (uint64_t)a->N};
   const uint64_t strB[1] = {K};
-  const uint32_t boxB[2] = {64u, (uint32_t)(BN / NCTA)};
+  const uint32_t boxB[2] = {64u, (uint32_t)BN};
   rc = cached_tmap_bf16(&p.mapB, a->B, 2, dimsB, strB, boxB, 128);
   if (rc != PN_OK) return rc;
 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-  if (halo_mode) return NCTA == 2 ? launch_gemm_mode<160, 10, 2, 6>(p, stream) : launch_gemm_mode<160, 5, 1, 6>(p, stream);
-  if (stream_mode && a->out_bf16) {
-#define PN_STREAM_BF16(M)                                                                                                   \
-    do {                                                                                                                    \
-      if (NCTA == 2) return BN == 160 ? launch_gemm_mode<160, 6, 2, M>(p, stream) : launch_gemm_mode<128, 7, 2, M>(p, stream); \
-      return BN == 160 ? launch_gemm_mode<160, 5, 1, M>(p, stream) : launch_gemm_mode<128, 6, 1, M>(p, stream);             \
-    } while (0)
-    if (a->ln_stats_in) PN_STREAM_BF16(8);
-    if (a->ln_stats_out) PN_STREAM_BF16(7);
-    PN_STREAM_BF16(5);
-#undef PN_STREAM_BF16
-  }
-  if (stream_mode) {
-    if (NCTA == 2) return BN == 160 ? launch_gemm_mode<160, 5, 2, 4>(p, stream) : launch_gemm_mode<128, 6, 2, 4>(p, stream);
-    return BN == 160 ? launch_gemm_mode<160, 4, 1, 4>(p, stream) : launch_gemm_mode<128, 5, 1, 4>(p, stream);
-  }
-  if (NCTA == 2 && BN == 192) return launch_gemm<192, 6, 2>(p, stream);
-  if (NCTA == 2 && BN == 128) return launch_gemm<128, 7, 2>(p, stream);
-  if (NCTA == 2 && BN == 64) return launch_gemm<64, 8, 2>(p, stream);
-  if (NCTA == 2) return BN == 256 ? launch_gemm<256, 6, 2>(p, stream) : launch_gemm<160, 7, 2>(p, stream);
+  const int mode = a->geglu ? 2 : a->out_bf16 ? 1 : 0;
   switch (BN) {
-    case 160: return launch_gemm<160, 5, 1>(p, stream);
-    case 128: return launch_gemm<128, 6, 1>(p, stream);
-    case 64: return launch_gemm<64, 8, 1>(p, stream);
-    default: return launch_gemm<32, 8, 1>(p, stream);
+    case 160: return launch_gemm<160, 5>(p, mode, tiles, stream);
+    case 128: return launch_gemm<128, 6>(p, mode, tiles, stream);
+    case 64: return launch_gemm<64, 8>(p, mode, tiles, stream);
+    default: return launch_gemm<32, 8>(p, mode, tiles, stream);
   }
 }
 
-// diagnostics (not part of the product ABI): role cycle counters of the last pn_gemm launch made with PN_GEMM_DEBUG=5
-extern "C" int pn_debug_gemm_counters(unsigned long long* out16) {
-  PN_CHECK_CUDA(cudaDeviceSynchronize());
-  PN_CHECK_CUDA(cudaMemcpyFromSymbol(out16, pn::g_gemm_dbg, sizeof(unsigned long long) * 16));
-  return PN_OK;
-}
-
-// number of partial (sum, sum of squares) pairs per row that a streaming bf16 pn_gemm with N output columns writes to
+// number of partial (sum, sum of squares) pairs per row that a bf16 pn_gemm with N output columns writes to
 // ln_stats_out (2 per 160- or 128-wide column tile)
 extern "C" int pn_gemm_ln_parts(int N) {
   if (N <= 0 || (N % 160 != 0 && N % 128 != 0)) return 0;

@@ -10,7 +10,7 @@ Step-invariant work is hoisted into `prepare_condition`: the BEV hint stem (cont
 K/V projections (attention.py:248-250), which the reference recomputes at every step — including 26.8 TFLOP of
 per-pixel repeated text K/V in the temporal blocks (attention.py:1122-1125) that simply never happens here.
 
-`ops` is `panacea_b200.ops.NativeOps` in production (hand-written sm_100a kernels). Tests inject a torch
+`ops` is `panacea_b200.ops.NativeOps` in production (hand-written sm_90a kernels). Tests inject a torch
 reference op set with the same interface to check this orchestration on CPU; the package itself has no fallback.
 """
 from __future__ import annotations
@@ -341,8 +341,8 @@ class Engine:
         y, st = ops.gemm(o.view(-1, C), W[t + ".attn1.o.w"], bias=W[t + ".attn1.o.b"], residual=y, out=y, out_dtype=y.dtype, ln_stats_out=True)
         q = ops.gemm(y, W[t + ".q2.w"], bias=W[t + ".q2.t"], out_dtype=dt, ln=(st, W[t + ".q2.s"], eps))
         o = ops.attention_text(q.view(b, T * H * Wd, C), kv, heads)
-        # norm3 stays a kernel: the GEGLU epilogue is the long pole of ff1 at level 0 and a rank-1 correction there cost it
-        # more (+2.7 ms per step) than the LayerNorm pass it saved (1.8 ms) — measured in round 2, profiles/README.md
+        # norm3 stays a kernel: the GEGLU epilogue is the long pole of ff1 at level 0, a rank-1 correction there would
+        # lengthen it
         y = ops.gemm(o.view(-1, C), W[t + ".attn2.o.w"], bias=W[t + ".attn2.o.b"], residual=y, out=y, out_dtype=y.dtype)
         n3 = ops.layernorm(y, W[t + ".norm3.g"], W[t + ".norm3.b"])
         ff = ops.gemm(n3, W[t + ".ff1.w"], bias=W[t + ".ff1.b"], geglu=True, out_dtype=ops.act_dtype)

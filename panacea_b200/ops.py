@@ -1,4 +1,4 @@
-"""Op layer: torch CUDA tensors in, hand-written sm_100a kernels (via the C ABI) out.
+"""Op layer: torch CUDA tensors in, hand-written sm_90a kernels (via the C ABI) out.
 
 Every method validates shapes/dtypes, builds the plain-C argument struct and launches on torch's current
 stream. No method computes anything in torch: torch is only the allocator and stream owner here.
@@ -62,7 +62,7 @@ class NativeOps:
     fused_operand_emit = True # a GEMM epilogue may store the next GEMM's operand directly (out_dtype=bf16)
     token_dtype = BF16        # token stream inside a transformer block (proj_in .. proj_out): 3 residual adds per block
     fold_layernorm = True     # LayerNorm folded into the GEMMs around the bf16 token stream (C <= LN_FOLD_MAX_C)
-    LN_FOLD_MAX_C = 640       # the producers' streaming bf16 epilogue (which emits the row sums) covers K <= 640
+    LN_FOLD_MAX_C = 640       # LayerNorm fold up to C = 640; wider token streams keep the LayerNorm kernel
 
     def __init__(self):
         import os
@@ -425,7 +425,7 @@ class NativeOps:
 class ParityOps(NativeOps):
     """fp32-class precision mode (the literal rtol 1e-3 / atol 1e-4 bar of BASELINE.json against the reference's fp32
     math). Same kernels, different operand encoding: every producer stores the GEMM operand as bf16 [hi | lo | hi]
-    (3C wide), weights are packed [W_hi | W_hi | W_lo], so the tcgen05 GEMM/conv kernel computes fp32-class products by
+    (3C wide), weights are packed [W_hi | W_hi | W_lo], so the wgmma GEMM/conv kernel computes fp32-class products by
     K-concatenation; attention runs in fp32 on CUDA cores (pn_attention_f32); GEGLU uses the exact erf; the
     time-embedding linears read fp32 weights. About 3-4x the cost of the bf16 path."""
 

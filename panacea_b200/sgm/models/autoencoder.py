@@ -72,7 +72,7 @@ class AutoencoderKLInferenceWrapper(nn.Module):
     @torch.no_grad()
     def encode_moments(self, x):
         if not x.is_cuda:
-            raise RuntimeError("panacea_b200 runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("panacea_b200 runs on CUDA (sm_90a) only; there is no CPU path")
         if self._enc_engine is None:
             from ...ops import NativeOps
             self._enc_engine = VAEEncoderEngine(self.ddconfig, NativeOps(), self.embed_dim)
@@ -92,9 +92,9 @@ class AutoencoderKLInferenceWrapper(nn.Module):
 
     @torch.no_grad()
     def decode(self, z):
-        """autoencoder.py:362-365 on the sm_100a kernels (no CPU path)."""
+        """autoencoder.py:362-365 on the sm_90a kernels (no CPU path)."""
         if not z.is_cuda:
-            raise RuntimeError("panacea_b200 runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("panacea_b200 runs on CUDA (sm_90a) only; there is no CPU path")
         if self._engine is None:
             from ...ops import NativeOps
             self._engine = VAEDecoderEngine(self.ddconfig, NativeOps(), self.embed_dim)

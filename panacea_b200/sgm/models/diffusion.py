@@ -2,7 +2,7 @@
 network + wrapper, denoiser, sampler, conditioner and first stage from the `model.params` block of
 configs/inference_nuscenes.yaml and runs the inference control flow `log_images -> sample -> decode_first_stage`
 (SURVEY.md section 8f, row N1). Training, EMA, optimisers and logging of text images are not part of the inference
-path and are not mirrored. The denoising loop inside `sample` is the hot path of this repository (sm_100a kernels)."""
+path and are not mirrored. The denoising loop inside `sample` is the hot path of this repository (sm_90a kernels)."""
 from __future__ import annotations
 
 import torch

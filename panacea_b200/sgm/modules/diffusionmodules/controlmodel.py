@@ -3,7 +3,7 @@
 
 Same constructor keywords, same `forward` signatures, same state-dict keys — but no nn.Module tree and no
 torch compute: parameters live in one flat table keyed by the reference's names, and `forward` runs the
-hand-written sm_100a kernels through `panacea_b200.engine.Engine`. Without the native library (or without a
+hand-written sm_90a kernels through `panacea_b200.engine.Engine`. Without the native library (or without a
 CUDA device) `forward` raises; there is no eager fallback.
 """
 from __future__ import annotations

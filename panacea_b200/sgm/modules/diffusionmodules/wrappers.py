@@ -88,7 +88,7 @@ class OpenAIWrapperControlLDM3D(IdentityWrapper):
     @torch.no_grad()
     def forward(self, x: torch.Tensor, t: torch.Tensor, c: dict, *, return_static: bool = False, **kwargs) -> torch.Tensor:
         if not x.is_cuda:
-            raise RuntimeError("panacea_b200 runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("panacea_b200 runs on CUDA (sm_90a) only; there is no CPU path")
         eng = self.diffusion_model.engine()
         self._ensure_prepared(eng, c)
         x = x.float().contiguous()

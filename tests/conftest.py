@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with `-m gpu` on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); select with `-m gpu`")
     config.addinivalue_line("markers", "slow: long-running CPU test")
 
 

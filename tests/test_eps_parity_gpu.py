@@ -3,7 +3,7 @@
  (b) the CPU oracle port run on this box on the same seeded inputs.
 
 Two precision modes, two bars:
- * "parity" (ParityOps: split-bf16 operands = fp32-class products on the same tcgen05 kernels, fp32 attention): the
+ * "parity" (ParityOps: split-bf16 operands = fp32-class products on the same wgmma kernels, fp32 attention): the
    LITERAL tolerance of BASELINE.json, rtol 1e-3 / atol 1e-4, on >= 99.9 % of the elements of every case, including the
    full-size model at the benchmarked shape [16, 8, 32, 336] (T = 8, CFG b = 2);
  * "bf16" (the benchmarked fast path: bf16 operands, fp32 accumulation / softmax / norm statistics / residual stream):

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 GEMM / implicit-conv kernel against torch fp32 math on the same bf16 inputs."""
+"""GPU parity of the wgmma GEMM / implicit-conv kernel against torch fp32 math on the same bf16 inputs."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -66,7 +66,7 @@ def test_gemm_bf16_out_and_rowvec(ops):
 @pytest.mark.parametrize("M,N,K", [(3000, 320, 320), (2048, 640, 640), (1500, 1280, 1280), (172032 // 4, 320, 1280), (130, 320, 320)])
 def test_gemm_bf16_token_stream_residual(ops, M, N, K):
     """bf16 output with a bf16 residual updated in place (the transformer blocks' token stream): streaming epilogue
-    (K <= 640, TMA-loaded residual tile) and the generic bf16 epilogue (larger K)."""
+    (K <= 640 and larger K)."""
     a = _rand((M, K), 13); w = _rand((N, K), 14, K ** -0.5)
     bias = _rand((N,), 15, dtype=torch.float32)
     y = _rand((M, N), 16)

@@ -62,7 +62,7 @@ def test_parity_mode_split_operands_reach_fp32_class_accuracy(name):
     """Parity mode on CPU: the engine packs weights [W_hi | W_hi | W_lo] and every producer stores [hi | lo | hi]
     (emulated by TorchSplitOps with exact bf16-value products). Against the reference golden the literal BASELINE
     tolerance rtol 1e-3 / atol 1e-4 must hold on (essentially) every element — the same packing runs on the GPU through
-    the tcgen05 kernel."""
+    the wgmma kernel."""
     case = [c for c in Cs.GOLDEN_CASES if c.name == name][0]
     cfg = NP.config_from_kwargs(case.unet_kwargs())
     eng = E.Engine(cfg, TorchSplitOps())
@@ -187,14 +187,14 @@ def test_geglu_pack_is_the_layout_the_epilogue_contract_states():
 
 def test_geglu_erfc_constants_in_the_kernel_source_are_accurate():
     """The GEGLU epilogue evaluates Phi(-t) = 0.5 * 2^(-t Q(t)) with a fitted degree-4 Q and NO clamp of t = |g|
-    (ptx.cuh::geglu_f32x2, generated by tools/fit_erfc.py). Re-evaluate the constants found in the kernel source in fp32
+    (ptx.cuh::geglu_f32, generated by tools/fit_erfc.py). Re-evaluate the constants found in the kernel source in fp32
     on the CPU against the exact erf GELU of the reference (attention.py:97-99 -> F.gelu), far beyond the fitted range too."""
     import re
     import numpy as np
     src = (Path(__file__).resolve().parent.parent / "panacea_b200" / "csrc" / "ptx.cuh").read_text()
-    body = src[src.index("__device__ __forceinline__ f32x2 geglu_f32x2"):]
+    body = src[src.index("__device__ __forceinline__ float geglu_f32"):]
     body = body[:body.index("\n}\n")]
-    coef = [float(x) for x in re.findall(r"f2_splat\((-?[0-9.]+e?[-+]?[0-9]*)f\)", body)]
+    coef = [float(x) for x in re.findall(r"(-?[0-9]+\.[0-9]+(?:e[-+]?[0-9]+)?)f\b", body)]
     # Horner order in the source: c4, c3, ..., c0, then the -0.5 / 0.5 / 0.5 of the final combination
     c = np.array(coef[:5], dtype=np.float32)
     assert len(coef) >= 5 and abs(c[-1] - 1.1510913) < 1e-6 and c[0] > 0          # positive leading coefficient: no clamp needed

@@ -80,7 +80,7 @@ def test_frame_writers_produce_the_streampetr_layout(tmp_path):
 @pytest.mark.gpu
 def test_inference_entry_point_end_to_end(tmp_path):
     """The whole main(): YAML -> engine -> DistributedSampler/bs=1 loop -> log_images (conditioner, VAE-stub encode,
-    share-noise init, 3 Euler/CFG steps on the sm_100a path, decode) -> writers."""
+    share-noise init, 3 Euler/CFG steps on the sm_90a path, decode) -> writers."""
     from panacea_b200 import inference as INF
     written = INF.main(["--name", "t", "--base", CFG, "--inferdir", str(tmp_path), "--num_sequences", "2", "--image_hw", "64", "128",
                         "--randomize_zero_init"])

@@ -1,5 +1,5 @@
 """GPU tests of the parity-mode building blocks (panacea_b200.ops.ParityOps) against float64 torch math:
-split-bf16 operands through the tcgen05 GEMM / implicit conv, the fp32 attention kernels (head_dim 64 and 80), the
+split-bf16 operands through the wgmma GEMM / implicit conv, the fp32 attention kernels (head_dim 64 and 80), the
 exact-erf GEGLU pass and the split stores of the normalisation kernels. Tolerances are fp32-class (1e-5 .. 1e-4)."""
 import pytest
 import torch

@@ -1,5 +1,5 @@
 """Merge tools/attn_sweep.py's CUDA-event timings with the ncu metrics pass of the same launches into the markdown table
-of profiles/r02_attn_sweep.md."""
+of the attention sweep report."""
 import csv
 import json
 import sys
@@ -35,4 +35,4 @@ for i, e in enumerate(ev):
           f"{'-' if tp is None else f'{tp:.1f}'} | {gbs:.0f} | {gbs / pk_bw:.3f} | {dr / 1e6:.0f} / {dw / 1e6:.0f} |")
 print(f"\nPeaks: MEASURED_PEAKS.json bf16 burst {pk_tf:.0f} TF/s, HBM copy {pk_bw:.0f} GB/s (of measured). FLOPs = 4 B heads Nq Nk d, "
       "bytes = 2 d B heads (2 Nq + 2 Nk) (SURVEY.md section 8d). The temporal kernel is the warp-level mma.sync kernel (T <= 16 rows cannot "
-      "fill a tcgen05 tile): it is HBM-bound, its tensor-pipe figure is not a target.")
+      "fill a wgmma tile): it is HBM-bound, its tensor-pipe figure is not a target.")

@@ -7,7 +7,8 @@
  *   sgm/modules/diffusionmodules/controlmodel.py:86-202 ControlNet3D / ControlledUNetModel3D.forward
  *   sgm/modules/diffusionmodules/openaimodel.py:499-542 ResBlock3D._forward
  *   sgm/modules/attention.py:407-610,229-291,1064-1134  view / text / temporal attention, STT
- *   sgm/modules/diffusionmodules/sampling.py:96-133     EulerEDMSampler step
+ *   sgm/modules/diffusionmodules/sampling.py:85-365     EDM (Euler with churn, Heun), ancestral (Euler-a,
+ *                                                       DPM++ 2S-a), DPM++ 2M and LMS solver steps
  * and every entry point below names the reference call site it replaces. The Python host
  * (panacea_b200/sgm/...) mirrors those classes and binds these symbols with ctypes (INTEGRATION.md).
  *
@@ -189,13 +190,6 @@ int pn_timestep_embedding(const int64_t* t, float* out, int64_t n, int64_t dim, 
  * (openaimodel.py:936-943, 439-445). */
 int pn_linear_small(const float* x, const void* W, int w_is_f32, const float* bias, float* y, int64_t M, int64_t N,
                     int64_t K, int64_t ldy, int silu_in, int silu_out, void* stream);
-/* One Euler step with classifier-free guidance, reference operation order (denoiser.py:22-28, guiders.py:25-29,
- * sampling_utils.py:7-9,39-40, sampling.py:103-110). net2 = [uncond ; cond] halves of n elements each: the network's
- * eps prediction (net_is_denoised = 0; the denoiser's c_out = -sigma_q, c_skip = 1 are applied here, sigma_q being
- * sigma snapped to the denoiser's 1000-entry table) or already-denoised samples (net_is_denoised = 1).
- * x is updated in place; x_in_next (optional, 2n elements) receives x_new * c_in_next duplicated. */
-int pn_cfg_euler_step(float* x, const float* net2, float* x_in_next, int64_t n, float sigma, float sigma_q,
-                      float sigma_next, float cfg_scale, float c_in_next, int net_is_denoised, void* stream);
 /* out[r, :] = softmax(scale * in[r, :]), fp32 scores -> bf16 probabilities. With two pn_gemm calls around it this is the
  * single-head attention of the VAE mid block (reference sgm/modules/diffusionmodules/model.py:374-414, head_dim = C). */
 int pn_softmax_rows(const float* in, void* out_bf16, int64_t rows, int64_t N, int64_t ld_in, int64_t ld_out, float scale,
@@ -206,6 +200,77 @@ int pn_softmax_rows(const float* in, void* out_bf16, int64_t rows, int64_t N, in
 int pn_fingerprint(const void* x, int64_t nbytes, uint64_t* out2, void* stream);
 /* out[c*n + i] = x[i] * s for c < copies (prepare_sampling_loop x *= sqrt(1+sigma0^2), CFG batch doubling). */
 int pn_scale_dup(const float* x, float* out, int64_t n, float s, int copies, void* stream);
+
+/* One Euler step with classifier-free guidance, reference operation order (denoiser.py:22-28, guiders.py:25-29,
+ * sampling_utils.py:7-9,39-40, sampling.py:103-110). net2 = [uncond ; cond] halves of n elements each: the network's
+ * eps prediction (net_is_denoised = 0; the denoiser's c_out = -sigma_q, c_skip = 1 are applied here, sigma_q being
+ * sigma snapped to the denoiser's 1000-entry table) or already-denoised samples (net_is_denoised = 1).
+ * x is updated in place; x_in_next (optional, 2n elements) receives x_new * c_in_next duplicated. Same kernel and
+ * arithmetic as pn_sampler_step in PN_SAMPLER_EULER mode with two halves and dt = sigma_next - sigma. */
+int pn_cfg_euler_step(float* x, const float* net2, float* x_in_next, int64_t n, float sigma, float sigma_q,
+                      float sigma_next, float cfg_scale, float c_in_next, int net_is_denoised, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * pn_sampler_step — one launch after every network evaluation of a sampler (sampling.py:85-365,
+ * sampling_utils.py:12-48), fp32, grid-stride, allocation-free. Per element, in the reference's fp32 order:
+ *   xe  = x_eval ? x_eval : x                         the point the network was evaluated at
+ *   D_h = net_is_denoised ? net_h : net_h * (-sigma_q) + xe      (denoiser.py:22-28, EpsScaling: c_skip 1, c_out -sigma_q)
+ *   D   = halves == 2 ? D_0 + cfg_scale (D_1 - D_0) : D_0       (VanillaCFG, unconditional half first; IdentityGuider)
+ *   o   = the mode's update (pn_sampler_mode)
+ *   o  += (xi * noise_scale) * noise_amp              when noise_amp != 0; xi = noise[e], or, with noise == NULL, the
+ *                                                     standard normal Philox4x32-10(key seed, counter (e / 4, draw)) +
+ *                                                     Box-Muller: a function of (seed, draw, e) only
+ *   out = o (out == NULL: x, in place);  x_in_next[h * n + e] = o * c_in_next for h < halves (when non-NULL).
+ * hist is a ring of n-element slots: the Heun predictor's d, the LMS d_{i-j}, the DPM++ 2M D_{i-1}. A slot may be read
+ * and written by the same launch (element-wise, read first).
+ * ---------------------------------------------------------------------------------------------- */
+enum pn_sampler_mode {
+  /* o = xe + dt * d, d = (xe - D) / sigma; hist[hist_write] = d. EulerEDMSampler and EDMSampler with churn
+   * (sampling.py:96-110, sigma = sigma_hat, dt = sigma_next - sigma_hat), HeunEDMSampler's predictor (out = stage
+   * buffer) and its last step, EulerAncestralSampler (:240-247, dt = sigma_down - sigma, noise_amp = sigma_up) and
+   * DPMPP2SAncestralSampler when sigma_down = 0 (:270-272). */
+  PN_SAMPLER_EULER = 0,
+  /* o = x + ((hist[hist_read[0]] + d') / 2) * dt, d' = (xe - D) / sigma: HeunEDMSampler's corrector (:229-235),
+   * evaluated at the predictor xe = stage, sigma = sigma_next. */
+  PN_SAMPLER_HEUN = 1,
+  /* o = x + (coef[0] d + sum_{j>=1} coef[j] hist[hist_read[j-1]]), d = (xe - D) / sigma, hist[hist_write] = d:
+   * LinearMultistepSampler (:194-209), coefficients from linear_multistep_coeff (sampling_utils.py:12-24). */
+  PN_SAMPLER_LMS = 2,
+  /* o = coef[0] x - coef[1] D; hist[hist_write] = D. DPMPP2SAncestralSampler's midpoint (:279, out = stage) and update
+   * (:281, evaluated at xe = stage), DPMPP2MSampler's x_standard (:332, first step and sigma_next = 0). */
+  PN_SAMPLER_DPM = 3,
+  /* o = coef[0] x - coef[1] (coef[2] D - coef[3] hist[hist_read[0]]); hist[hist_write] = D: DPMPP2MSampler (:337-338). */
+  PN_SAMPLER_DPM_2M = 4,
+  /* o = coef[0] x, no network term (net unused): prepare_sampling_loop's x *= sqrt(1 + sigma_0^2) (:50), plus the
+   * churn noise of step 0 and the first network input. */
+  PN_SAMPLER_SCALE = 5
+};
+
+typedef struct pn_sampler_step_args {
+  float* x;                 /* [n] sampler state */
+  const float* x_eval;      /* [n] evaluation point, or NULL = x */
+  const float* net;         /* [halves * n] network output (eps; or D when net_is_denoised) */
+  float* out;               /* [n] destination of o, or NULL = x (may alias x or x_eval) */
+  float* hist;              /* [slots * n] history ring, or NULL */
+  const float* noise;       /* [n] caller's standard-normal draws, or NULL = in-kernel Philox */
+  float* x_in_next;         /* [halves * n] next network input, or NULL */
+  int64_t n;                /* elements of one half */
+  uint64_t seed, draw;      /* Philox key and draw index */
+  int32_t mode;             /* pn_sampler_mode */
+  int32_t halves;           /* 2: VanillaCFG, 1: IdentityGuider */
+  int32_t net_is_denoised;
+  int32_t hist_read[3];     /* slots read (HEUN, DPM_2M: [0]; LMS: d_{i-1}, d_{i-2}, d_{i-3}); -1 = none */
+  int32_t hist_write;       /* slot written (d or D, see the modes); -1 = none */
+  float sigma_q;            /* sigma snapped to the denoiser's table: c_out = -sigma_q */
+  float cfg_scale;
+  float sigma;              /* divisor of to_d */
+  float dt;
+  float coef[4];            /* LMS coefficients / DPM++ multipliers / SCALE factor */
+  float noise_scale, noise_amp;
+  float c_in_next;          /* c_in of the next evaluation's quantised sigma */
+} pn_sampler_step_args;
+
+int pn_sampler_step(const pn_sampler_step_args* args, void* stream);
 
 #ifdef __cplusplus
 }

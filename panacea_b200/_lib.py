@@ -45,6 +45,18 @@ class AttnArgs(C.Structure):
     ]
 
 
+class SamplerStepArgs(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("x_eval", C.c_void_p), ("net", C.c_void_p), ("out", C.c_void_p), ("hist", C.c_void_p),
+        ("noise", C.c_void_p), ("x_in_next", C.c_void_p),
+        ("n", C.c_int64), ("seed", C.c_uint64), ("draw", C.c_uint64),
+        ("mode", C.c_int32), ("halves", C.c_int32), ("net_is_denoised", C.c_int32),
+        ("hist_read", C.c_int32 * 3), ("hist_write", C.c_int32),
+        ("sigma_q", C.c_float), ("cfg_scale", C.c_float), ("sigma", C.c_float), ("dt", C.c_float),
+        ("coef", C.c_float * 4), ("noise_scale", C.c_float), ("noise_amp", C.c_float), ("c_in_next", C.c_float),
+    ]
+
+
 _vp, _i64, _i32, _f32 = C.c_void_p, C.c_int64, C.c_int32, C.c_float
 
 # name -> (restype, argtypes); every symbol declared in include/panacea_b200.h must appear here
@@ -74,6 +86,7 @@ SIGNATURES: dict[str, tuple] = {
     "pn_timestep_embedding": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
     "pn_linear_small": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _i64, _i64, _i64, _i64, C.c_int, C.c_int, _vp]),
     "pn_cfg_euler_step": (C.c_int, [_vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _f32, C.c_int, _vp]),
+    "pn_sampler_step": (C.c_int, [C.POINTER(SamplerStepArgs), _vp]),
     "pn_scale_dup": (C.c_int, [_vp, _vp, _i64, _f32, C.c_int, _vp]),
     "pn_fingerprint": (C.c_int, [_vp, _i64, _vp, _vp]),
     "pn_softmax_rows": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _f32, _vp]),

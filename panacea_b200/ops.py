@@ -14,6 +14,8 @@ from . import _lib
 BF16 = torch.bfloat16
 F32 = torch.float32
 OP_BF16, OP_SPLIT3, OP_F32 = 0, 1, 2      # include/panacea_b200.h pn_operand_mode
+# include/panacea_b200.h pn_sampler_mode
+SAMPLER_EULER, SAMPLER_HEUN, SAMPLER_LMS, SAMPLER_DPM, SAMPLER_DPM_2M, SAMPLER_SCALE = range(6)
 
 
 def _ptr(t):
@@ -395,6 +397,38 @@ class NativeOps:
                                              _stream()), "pn_cfg_euler_step")
         self.launches += 1
         return x
+
+    def sampler_step(self, mode, x, net=None, *, x_eval=None, out=None, hist=None, noise=None, x_in_next=None, halves=2,
+                     net_is_denoised=False, sigma_q=0.0, cfg_scale=1.0, sigma=0.0, dt=0.0, coef=(), hist_read=(),
+                     hist_write=-1, noise_scale=1.0, noise_amp=0.0, seed=0, draw=0, c_in_next=0.0):
+        """One pn_sampler_step launch (include/panacea_b200.h): the update of `mode` from the network output `net`
+        [halves * n] evaluated at `x_eval` (None: x), written to `out` (None: x, in place), plus optional noise
+        (`noise` [n], or the in-kernel Philox stream (seed, draw) when None) and the next network input. fp32 in both
+        precision modes. Returns the destination tensor."""
+        n = x.numel()
+        _req(x.dtype == F32 and x.is_contiguous(), "sampler_step: x must be contiguous fp32")
+        for name, t, size in (("net", net, halves * n), ("x_eval", x_eval, n), ("out", out, n), ("noise", noise, n),
+                              ("x_in_next", x_in_next, halves * n)):
+            _req(t is None or (t.dtype == F32 and t.is_contiguous() and t.numel() == size and t.device == x.device),
+                 f"sampler_step: {name} must be contiguous fp32 with {size} elements on x's device")
+        _req(hist is None or (hist.dtype == F32 and hist.is_contiguous() and hist.numel() % n == 0), "sampler_step: hist slots")
+        slots = 0 if hist is None else hist.numel() // n
+        _req(all(-1 <= r < slots for r in hist_read) and -1 <= hist_write < max(slots, 0), "sampler_step: hist slot out of range")
+        a = _lib.SamplerStepArgs()
+        a.x, a.x_eval, a.net, a.out = x.data_ptr(), _ptr(x_eval), _ptr(net), _ptr(out)
+        a.hist, a.noise, a.x_in_next = _ptr(hist), _ptr(noise), _ptr(x_in_next)
+        a.n, a.seed, a.draw = n, int(seed), int(draw)
+        a.mode, a.halves, a.net_is_denoised = int(mode), int(halves), int(bool(net_is_denoised))
+        for j in range(3):
+            a.hist_read[j] = hist_read[j] if j < len(hist_read) else -1
+        a.hist_write = hist_write
+        a.sigma_q, a.cfg_scale, a.sigma, a.dt = float(sigma_q), float(cfg_scale), float(sigma), float(dt)
+        for j, v in enumerate(coef):
+            a.coef[j] = float(v)
+        a.noise_scale, a.noise_amp, a.c_in_next = float(noise_scale), float(noise_amp), float(c_in_next)
+        _lib.check(self.lib.pn_sampler_step(C.byref(a), _stream()), "pn_sampler_step")
+        self.launches += 1
+        return x if out is None else out
 
     def softmax_rows(self, s, scale):
         """fp32 [rows, N] -> bf16 [rows, N] = softmax(scale * s) per row (VAE mid-block attention)."""

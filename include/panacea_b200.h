@@ -134,6 +134,17 @@ int pn_attention_temporal_f32(const float* q, const float* k, const float* v, vo
                               int64_t pixels, int32_t heads, int32_t head_dim, int64_t ld, float scale, int operand_mode,
                               void* stream);
 
+/* Causal self-attention of the OpenCLIP text transformer (reference sgm/modules/encoders/modules.py:618-629, each
+ * resblock's nn.MultiheadAttention with attn_mask = -inf above the diagonal: token i attends keys j <= i).
+ * q/k/v bf16 [batch, L, ld] (e.g. three base pointers into the fused in_proj output), out bf16 [batch, L, out_ld];
+ * L <= 128, head_dim 64, ld and out_ld multiples of 8. One CTA per (batch, head), warp-level bf16 MMAs, fp32 softmax. */
+int pn_attention_causal(const void* q, const void* k, const void* v, void* out, int64_t batch, int64_t L, int32_t heads,
+                        int32_t head_dim, int64_t ld, int64_t out_ld, float scale, void* stream);
+/* Parity-mode twin of pn_attention_causal (same call site): q/k/v fp32 [batch, L, ld], fp32 math on CUDA cores, `out`
+ * written as the out_proj GEMM operand [batch*L, heads*64] in `operand_mode`. */
+int pn_attention_causal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t L,
+                            int32_t heads, int32_t head_dim, int64_t ld, float scale, int operand_mode, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Normalisation (fp32 residual stream in, bf16 MMA operand out)
  * ---------------------------------------------------------------------------------------------- */
@@ -179,6 +190,13 @@ int pn_cast_operand(const float* x, void* y, int64_t rows, int64_t C, int operan
 /* Parity-mode GEGLU (attention.py:97-99, exact erf GELU) on the fp32 output of the ff.net.0 GEMM whose columns are in
  * pn_gemm's GEGLU packing (blocks of 32 = 16 value + 16 gate columns): in fp32 [rows, 2*inner] -> operand [rows, inner]. */
 int pn_geglu_operand(const float* in, void* y, int64_t rows, int64_t inner, int operand_mode, void* stream);
+/* y = 0.5 x (1 + erf(x / sqrt 2)): the exact GELU of the OpenCLIP text MLP (reference modules.py:618-629, resblock
+ * mlp = c_fc, GELU, c_proj), fp32 [rows, C] (the c_fc output) -> operand of the c_proj GEMM. */
+int pn_gelu_operand(const float* x, void* y, int64_t rows, int64_t C, int operand_mode, void* stream);
+/* out[b, l, :] = table[tokens[b, l], :] + pos[l, :], fp32 (reference modules.py:610-611, token_embedding +
+ * positional_embedding). The caller range-checks the int64 ids against vocab; an id outside [0, vocab) gives NaN. */
+int pn_token_embedding(const int64_t* tokens, const float* table, const float* pos, float* out, int64_t batch, int64_t L,
+                       int64_t vocab, int64_t width, void* stream);
 /* in[batch, A, first B of in_ld columns] -> out[batch, B, ld] at column offset off: NCHW <-> channels-last at the module
  * boundary (also performs the channel concat of wrappers.py:41, and drops the padding columns of the out-head GEMM). */
 int pn_transpose_f32(const float* in, float* out, int64_t batch, int64_t A, int64_t B, int64_t in_ld, int64_t out_ld,

@@ -70,6 +70,8 @@ SIGNATURES: dict[str, tuple] = {
     "pn_attention_temporal": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i64, _i64, _f32, _vp]),
     "pn_attention_f32": (C.c_int, [C.POINTER(AttnArgs), C.c_int, _vp]),
     "pn_attention_temporal_f32": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i64, _f32, C.c_int, _vp]),
+    "pn_attention_causal": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i64, _i64, _f32, _vp]),
+    "pn_attention_causal_f32": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i64, _f32, C.c_int, _vp]),
     "pn_groupnorm_workspace_floats": (_i64, [_i64, _i64, _i64]),
     "pn_groupnorm_silu": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _f32, C.c_int, C.c_int, _vp]),
     "pn_groupnorm_pixel_silu": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _f32, C.c_int, C.c_int, _vp]),
@@ -82,6 +84,8 @@ SIGNATURES: dict[str, tuple] = {
     "pn_add_inplace": (C.c_int, [_vp, _vp, _i64, _vp]),
     "pn_cast_operand": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int, _vp]),
     "pn_geglu_operand": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int, _vp]),
+    "pn_gelu_operand": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int, _vp]),
+    "pn_token_embedding": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _vp]),
     "pn_transpose_f32": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _i64, _i64, _vp]),
     "pn_timestep_embedding": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
     "pn_linear_small": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _i64, _i64, _i64, _i64, C.c_int, C.c_int, _vp]),

@@ -176,9 +176,86 @@ __global__ void __launch_bounds__(128) attn_f32_temporal_kernel(const float* __r
   }
 }
 
+// Causal self-attention (the OpenCLIP text transformer) in fp32: one thread per (batch, head, query i) visits keys
+// j <= i of its sequence, read from global/L1. Two passes over the keys (row maximum, then exp2 and P V) keep the
+// scores out of registers for L up to 128.
+// q/k/v fp32 [batch, L, ld] -> out operand [batch*L, heads*64]
+template <int OP>
+__global__ void __launch_bounds__(128) attn_f32_causal_kernel(const float* __restrict__ q, const float* __restrict__ k,
+                                                              const float* __restrict__ v, void* __restrict__ out, int batch,
+                                                              int L, int heads, long long ld, float scale_log2) {
+  constexpr int D = 64;
+  pdl_prologue_done();
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long total = (long long)batch * heads * L;
+  if (idx >= total) return;
+  const int qi = (int)(idx % L);
+  long long r = idx / L;
+  const int head = (int)(r % heads);
+  const int b = (int)(r / heads);
+  const long long row0 = (long long)b * L;
+  float qq[D], o[D];
+  const float* qp = q + (row0 + qi) * ld + head * D;
+#pragma unroll
+  for (int d = 0; d < D; d += 4) {
+    const float4 t = *reinterpret_cast<const float4*>(qp + d);
+    qq[d] = t.x * scale_log2; qq[d + 1] = t.y * scale_log2; qq[d + 2] = t.z * scale_log2; qq[d + 3] = t.w * scale_log2;
+  }
+  auto score = [&](int j) {
+    const float* kp = k + (row0 + j) * ld + head * D;
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+#pragma unroll
+    for (int d = 0; d < D; d += 4) {
+      const float4 kk = *reinterpret_cast<const float4*>(kp + d);
+      a0 = fmaf(qq[d], kk.x, a0); a1 = fmaf(qq[d + 1], kk.y, a1); a2 = fmaf(qq[d + 2], kk.z, a2); a3 = fmaf(qq[d + 3], kk.w, a3);
+    }
+    return (a0 + a1) + (a2 + a3);
+  };
+  float m = -INFINITY;
+  for (int j = 0; j <= qi; ++j) m = fmaxf(m, score(j));
+#pragma unroll
+  for (int d = 0; d < D; ++d) o[d] = 0.f;
+  float l = 0.f;
+  for (int j = 0; j <= qi; ++j) {
+    const float pj = exp2f(score(j) - m);
+    l += pj;
+    const float* vp = v + (row0 + j) * ld + head * D;
+#pragma unroll
+    for (int d = 0; d < D; d += 4) {
+      const float4 vv = *reinterpret_cast<const float4*>(vp + d);
+      o[d] = fmaf(pj, vv.x, o[d]); o[d + 1] = fmaf(pj, vv.y, o[d + 1]); o[d + 2] = fmaf(pj, vv.z, o[d + 2]); o[d + 3] = fmaf(pj, vv.w, o[d + 3]);
+    }
+  }
+  const float inv = 1.f / l;
+#pragma unroll
+  for (int d = 0; d < D; d += 8) {
+    const float v8[8] = {o[d] * inv, o[d + 1] * inv, o[d + 2] * inv, o[d + 3] * inv,
+                         o[d + 4] * inv, o[d + 5] * inv, o[d + 6] * inv, o[d + 7] * inv};
+    store_op8<OP>(out, (size_t)(row0 + qi), heads * D, head * D + d, v8);
+  }
+}
+
 }  // namespace pn
 
 using namespace pn;
+
+extern "C" int pn_attention_causal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t L,
+                                       int32_t heads, int32_t head_dim, int64_t ld, float scale, int operand_mode,
+                                       void* stream_v) {
+  PN_REQUIRE(q && k && v && out, "pn_attention_causal_f32: null pointer");
+  PN_REQUIRE(head_dim == 64, "pn_attention_causal_f32: head_dim %d unsupported (64)", head_dim);
+  PN_REQUIRE(batch > 0 && L >= 1 && L <= 128 && heads > 0, "pn_attention_causal_f32: bad geometry (1 <= L <= 128)");
+  PN_REQUIRE(ld % 4 == 0 && ld >= (int64_t)heads * head_dim, "pn_attention_causal_f32: bad token stride");
+  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_attention_causal_f32: operand_mode %d", operand_mode);
+  const long long total = batch * heads * L;
+  const long long blocks = (total + 127) / 128;
+  PN_REQUIRE(blocks < (1ll << 31), "pn_attention_causal_f32: grid too large");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+  PN_DISPATCH_OP(operand_mode, (launch_kernel(attn_f32_causal_kernel<OP>, dim3((unsigned)blocks), dim3(128), 0, st, 1, q, k, v, out,
+                                              (int)batch, (int)L, heads, ld, scale * 1.4426950408889634f)));
+  PN_CHECK_CUDA(cudaGetLastError());
+  return PN_OK;
+}
 
 extern "C" int pn_attention_f32(const pn_attn_args* a, int operand_mode, void* stream_v) {
   if (a == nullptr) return fail(PN_ERR_INVALID, "pn_attention_f32: null args");

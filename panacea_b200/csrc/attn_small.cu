@@ -141,9 +141,157 @@ __global__ void __launch_bounds__(TA_WARPS * 32) attn_temporal_kernel(const __nv
   }
 }
 
+// Causal self-attention over one short sequence per (batch, head): the text transformer of the OpenCLIP embedder
+// (open_clip ResidualAttentionBlock with attn_mask = -inf above the diagonal, L = 77). One CTA per (batch, head) stages
+// the L <= 128 rows of q, k and v once in shared memory; warp w owns query rows [16 w, 16 w + 16) and only visits the
+// key tiles its rows can see (keys <= its last row). S = Q K^T, the masked fp32 softmax and O = P V follow the
+// temporal kernel above, with P fed back as the A operand in chunks of 16 keys.
+constexpr int CA_MAXL = 128;
+constexpr int CA_D = 64;
+constexpr int CA_PITCH = CA_D + 8;
+
+__global__ void __launch_bounds__((CA_MAXL / 16) * 32) attn_causal_kernel(const __nv_bfloat16* __restrict__ q,
+                                                                          const __nv_bfloat16* __restrict__ k,
+                                                                          const __nv_bfloat16* __restrict__ v,
+                                                                          __nv_bfloat16* __restrict__ out, int L, int heads,
+                                                                          long long ld, long long out_ld, float scale) {
+  pdl_prologue_done();
+  constexpr int RCH = CA_D / 8;
+  extern __shared__ __align__(16) unsigned char ca_smem[];
+  const int Lp = (L + 15) & ~15;
+  __nv_bfloat16 (*sq)[CA_PITCH] = reinterpret_cast<__nv_bfloat16 (*)[CA_PITCH]>(ca_smem);   // Q rows, later the output
+  __nv_bfloat16 (*sk)[CA_PITCH] = sq + Lp;
+  __nv_bfloat16 (*sv)[CA_PITCH] = sk + Lp;
+  const int head = blockIdx.x % heads, b = blockIdx.x / heads;
+  const long long row0 = (long long)b * L;
+  // rows L..Lp-1 are MMA padding: they must be finite (0 * NaN would poison the valid rows of P V)
+  for (int i = threadIdx.x; i < Lp * RCH; i += blockDim.x) {
+    const int t = i / RCH, ch = i % RCH;
+    uint4 zq = make_uint4(0, 0, 0, 0), zk = zq, zv = zq;
+    if (t < L) {
+      const long long off = (row0 + t) * ld + head * CA_D + ch * 8;
+      zq = *reinterpret_cast<const uint4*>(q + off);
+      zk = *reinterpret_cast<const uint4*>(k + off);
+      zv = *reinterpret_cast<const uint4*>(v + off);
+    }
+    *reinterpret_cast<uint4*>(&sq[t][ch * 8]) = zq;
+    *reinterpret_cast<uint4*>(&sk[t][ch * 8]) = zk;
+    *reinterpret_cast<uint4*>(&sv[t][ch * 8]) = zv;
+  }
+  __syncthreads();
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int qb = w * 16;                                    // first query row of this warp
+  const int ntile = min((L + 7) / 8, (qb + 16) / 8);        // key tiles of 8 that hold a key some row here may see
+  const int r0 = qb + (lane >> 2), cq = (lane & 3) * 2;     // accumulator fragment: rows r0, r0+8; columns cq, cq+1
+
+  // ---- S = Q K^T (16 x 8*ntile), fp32
+  float sacc[CA_MAXL / 8][4];
+#pragma unroll
+  for (int nt = 0; nt < CA_MAXL / 8; ++nt) sacc[nt][0] = sacc[nt][1] = sacc[nt][2] = sacc[nt][3] = 0.f;
+#pragma unroll
+  for (int kk = 0; kk < CA_D / 16; ++kk) {
+    uint32_t aq[4];
+    ldmatrix_x4(aq, &sq[qb + (lane & 15)][kk * 16 + (lane >> 4) * 8]);
+#pragma unroll
+    for (int nt = 0; nt < CA_MAXL / 8; ++nt) {
+      if (nt < ntile) {
+        uint32_t bk[2];
+        ldmatrix_x2(bk, &sk[nt * 8 + (lane & 7)][kk * 16 + ((lane >> 3) & 1) * 8]);
+        mma_16816(sacc[nt], aq, bk);
+      }
+    }
+  }
+  // ---- causal mask (key > query, key >= L, unvisited tiles) and softmax on the fragment
+  const float c = scale * 1.4426950408889634f;
+  float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+  for (int nt = 0; nt < CA_MAXL / 8; ++nt) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int key = nt * 8 + cq + e;
+      const bool vis = nt < ntile && key < L;
+      if (!(vis && key <= r0)) sacc[nt][e] = -INFINITY;
+      if (!(vis && key <= r0 + 8)) sacc[nt][2 + e] = -INFINITY;
+      mx0 = fmaxf(mx0, sacc[nt][e]);
+      mx1 = fmaxf(mx1, sacc[nt][2 + e]);
+    }
+  }
+  // every row sees key 0, so both maxima are finite
+  mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+  mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+  float sum0 = 0.f, sum1 = 0.f;
+#pragma unroll
+  for (int nt = 0; nt < CA_MAXL / 8; ++nt) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      sacc[nt][e] = ex2_approx((sacc[nt][e] - mx0) * c);            // exp2(-inf) = 0 for the masked keys
+      sacc[nt][2 + e] = ex2_approx((sacc[nt][2 + e] - mx1) * c);
+      sum0 += sacc[nt][e];
+      sum1 += sacc[nt][2 + e];
+    }
+  }
+  sum0 += __shfl_xor_sync(0xffffffffu, sum0, 1); sum0 += __shfl_xor_sync(0xffffffffu, sum0, 2);
+  sum1 += __shfl_xor_sync(0xffffffffu, sum1, 1); sum1 += __shfl_xor_sync(0xffffffffu, sum1, 2);
+  const float inv0 = 1.f / sum0, inv1 = 1.f / sum1;
+  // ---- O = P V (16 x 64): chunks of 16 keys, the S fragments of two key tiles form the A fragment of P
+  float o[CA_D / 8][4];
+#pragma unroll
+  for (int nd = 0; nd < CA_D / 8; ++nd) o[nd][0] = o[nd][1] = o[nd][2] = o[nd][3] = 0.f;
+  const int nchunk = (ntile + 1) / 2;
+#pragma unroll
+  for (int kc = 0; kc < CA_MAXL / 16; ++kc) {
+    if (kc < nchunk) {
+      const uint32_t ap[4] = {pack_bf16x2(sacc[2 * kc][0], sacc[2 * kc][1]), pack_bf16x2(sacc[2 * kc][2], sacc[2 * kc][3]),
+                              pack_bf16x2(sacc[2 * kc + 1][0], sacc[2 * kc + 1][1]),
+                              pack_bf16x2(sacc[2 * kc + 1][2], sacc[2 * kc + 1][3])};
+#pragma unroll
+      for (int nd = 0; nd < CA_D / 8; ++nd) {
+        uint32_t bv[2];
+        ldmatrix_x2_trans(bv, &sv[kc * 16 + (lane & 15)][nd * 8]);
+        mma_16816(o[nd], ap, bv);
+      }
+    }
+  }
+  __syncwarp();                                 // every lane has read its Q fragments: its 16 sq rows become the output
+#pragma unroll
+  for (int nd = 0; nd < CA_D / 8; ++nd) {
+    *reinterpret_cast<uint32_t*>(&sq[r0][nd * 8 + cq]) = pack_bf16x2(o[nd][0] * inv0, o[nd][1] * inv0);
+    *reinterpret_cast<uint32_t*>(&sq[r0 + 8][nd * 8 + cq]) = pack_bf16x2(o[nd][2] * inv1, o[nd][3] * inv1);
+  }
+  __syncwarp();
+  for (int i = lane; i < 16 * RCH; i += 32) {
+    const int t = qb + i / RCH, ch = i % RCH;
+    if (t < L)
+      *reinterpret_cast<uint4*>(out + (row0 + t) * out_ld + head * CA_D + ch * 8) = *reinterpret_cast<const uint4*>(&sq[t][ch * 8]);
+  }
+}
+
 }  // namespace pn
 
 using namespace pn;
+
+extern "C" int pn_attention_causal(const void* q, const void* k, const void* v, void* out, int64_t batch, int64_t L,
+                                   int32_t heads, int32_t head_dim, int64_t ld, int64_t out_ld, float scale, void* stream_v) {
+  PN_REQUIRE(q && k && v && out, "pn_attention_causal: null pointer");
+  PN_REQUIRE(head_dim == CA_D, "pn_attention_causal: head_dim %d unsupported (64)", head_dim);
+  PN_REQUIRE(L >= 1 && L <= CA_MAXL, "pn_attention_causal: L=%lld out of range 1..128", (long long)L);
+  PN_REQUIRE(batch > 0 && heads > 0 && ld % 8 == 0 && out_ld % 8 == 0 && ld >= (int64_t)heads * head_dim &&
+                 out_ld >= (int64_t)heads * head_dim,
+             "pn_attention_causal: bad arguments (ld and out_ld multiples of 8, >= heads*64)");
+  PN_REQUIRE(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+               reinterpret_cast<uintptr_t>(out)) & 15) == 0, "pn_attention_causal: pointers must be 16-byte aligned");
+  const long long blocks = batch * heads;
+  PN_REQUIRE(blocks < (1ll << 31), "pn_attention_causal: grid too large");
+  const int Lp = (int)((L + 15) & ~15);
+  const size_t smem = (size_t)3 * Lp * CA_PITCH * sizeof(__nv_bfloat16);
+  const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(&attn_causal_kernel), smem);
+  if (rc != PN_OK) return rc;
+  launch_kernel(attn_causal_kernel, dim3((unsigned)blocks), dim3((Lp / 16) * 32), smem, reinterpret_cast<cudaStream_t>(stream_v), 1,
+                reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
+                reinterpret_cast<const __nv_bfloat16*>(v), reinterpret_cast<__nv_bfloat16*>(out), (int)L, heads, ld, out_ld, scale);
+  PN_CHECK_CUDA(cudaGetLastError());
+  return PN_OK;
+}
 
 extern "C" int pn_attention_temporal(const void* q, const void* k, const void* v, void* out, int64_t batch, int64_t T,
                                      int64_t pixels, int32_t heads, int32_t head_dim, int64_t ld, int64_t out_ld,

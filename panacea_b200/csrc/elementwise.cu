@@ -118,6 +118,46 @@ __global__ void geglu_operand_kernel(const float* __restrict__ in, void* __restr
   }
 }
 
+// exact erf GELU of the OpenCLIP text MLP (nn.GELU between c_fc and c_proj): fp32 [rows, C] -> operand [rows, C]
+template <int OP>
+__global__ void gelu_operand_kernel(const float* __restrict__ x, void* __restrict__ y, size_t rows, int C) {
+  pdl_prologue_done();
+  const int c4n = C / 4;
+  const size_t n4 = rows * (size_t)c4n;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n4; e += (size_t)gridDim.x * blockDim.x) {
+    const float4 a = reinterpret_cast<const float4*>(x)[e];
+    const float in[4] = {a.x, a.y, a.z, a.w};
+    float o[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) o[i] = 0.5f * in[i] * (1.0f + erff(in[i] * 0.70710678118654752f));
+    store_op4<OP>(y, e / c4n, C, (int)(e % c4n) * 4, o);
+  }
+}
+
+// out[b, l, :] = table[tok[b, l], :] + pos[l, :] (OpenCLIP token_embedding + positional_embedding), fp32. The host
+// range-checks the ids; an id outside [0, vocab) that slips through yields NaN rows instead of an out-of-bounds read.
+__global__ void token_embedding_kernel(const long long* __restrict__ tok, const float* __restrict__ table,
+                                       const float* __restrict__ pos, float* __restrict__ out, size_t rows, int L,
+                                       long long vocab, int width) {
+  pdl_prologue_done();
+  const int c4n = width / 4;
+  const size_t n4 = rows * (size_t)c4n;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n4; e += (size_t)gridDim.x * blockDim.x) {
+    const size_t row = e / c4n;
+    const int c = (int)(e % c4n) * 4;
+    const long long t = tok[row];
+    const float4 p = *reinterpret_cast<const float4*>(pos + (size_t)(row % L) * width + c);
+    float4 r;
+    if (t >= 0 && t < vocab) {
+      const float4 w = *reinterpret_cast<const float4*>(table + (size_t)t * width + c);
+      r = make_float4(w.x + p.x, w.y + p.y, w.z + p.z, w.w + p.w);
+    } else {
+      r = make_float4(NAN, NAN, NAN, NAN);
+    }
+    *reinterpret_cast<float4*>(out + row * width + c) = r;
+  }
+}
+
 // ---------------------------------------------------------------- sinusoidal timestep embedding
 // util.py:224-248: emb[n] = [cos(t f_k), sin(t f_k)], f_k = exp(-ln(10000) k / half)
 // freqs (optional): the caller's fp32 table of the dim/2 frequencies (the host computes it with the reference's own
@@ -377,6 +417,27 @@ extern "C" int pn_geglu_operand(const float* in, void* y, int64_t rows, int64_t 
   const size_t n4 = (size_t)rows * (size_t)(inner / 4);
   PN_DISPATCH_OP(operand_mode, (launch_kernel(geglu_operand_kernel<OP>, dim3(grid_for(n4)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream_v), 1, 
       in, y, (size_t)rows, (int)inner)));
+  PN_CHECK_CUDA(cudaGetLastError());
+  return PN_OK;
+}
+
+extern "C" int pn_gelu_operand(const float* x, void* y, int64_t rows, int64_t C, int operand_mode, void* stream_v) {
+  PN_REQUIRE(x && y && rows > 0 && C > 0 && C % 4 == 0, "pn_gelu_operand: bad arguments");
+  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_gelu_operand: operand_mode %d", operand_mode);
+  const size_t n4 = (size_t)rows * (size_t)(C / 4);
+  PN_DISPATCH_OP(operand_mode, (launch_kernel(gelu_operand_kernel<OP>, dim3(grid_for(n4)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream_v), 1,
+      x, y, (size_t)rows, (int)C)));
+  PN_CHECK_CUDA(cudaGetLastError());
+  return PN_OK;
+}
+
+extern "C" int pn_token_embedding(const int64_t* tokens, const float* table, const float* pos, float* out, int64_t batch,
+                                  int64_t L, int64_t vocab, int64_t width, void* stream_v) {
+  PN_REQUIRE(tokens && table && pos && out, "pn_token_embedding: null pointer");
+  PN_REQUIRE(batch > 0 && L > 0 && vocab > 0 && width > 0 && width % 4 == 0, "pn_token_embedding: bad arguments");
+  const size_t n4 = (size_t)batch * (size_t)L * (size_t)(width / 4);
+  launch_kernel(token_embedding_kernel, dim3(grid_for(n4)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream_v), 1,
+                reinterpret_cast<const long long*>(tokens), table, pos, out, (size_t)(batch * L), (int)L, (long long)vocab, (int)width);
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }

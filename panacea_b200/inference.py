@@ -4,11 +4,15 @@ model built from `configs/inference_nuscenes.yaml`-style YAML via instantiate_fr
 writers. SURVEY.md section 8f rows N1 (engine / conditioner glue) and N3 (writers, gather -> rank-0 writer).
 
 What is NOT here, and why: the nuScenes dataset + BEV rasteriser (row N4, needs nuScenes and mmdet3d) is replaced by
-`SyntheticBEVDataset` with the same batch contract; the CLIP text tower is a deterministic stand-in (BASELINE.json
-configs[3]); the VAE (encoder and decoder) is native and random-init unless a checkpoint provides `first_stage_model.*`.
-With the real modules importable, `--dataset module:Class` and the YAML targets swap them in.
+`SyntheticBEVDataset` with the same batch contract. The VAE (encoder and decoder) is native and random-init unless a
+checkpoint provides `first_stage_model.*`. The OpenCLIP text tower is native too once it has weights: from the checkpoint
+(`conditioner.embedders.0.model.*`) or from a stock open_clip file given as the embedder's `version`; prompts are
+tokenized with the CLIP BPE vocabulary at the embedder's `bpe_path` (else open_clip's bundled copy). Without weights the
+embedder is a deterministic stand-in. With the real modules importable, `--dataset module:Class` and the YAML targets
+swap them in. Overrides use the dotlist form, and a numeric component indexes a list:
 
   torchrun --nproc-per-node 8 -m panacea_b200.inference --base configs.yaml --name run1 --inferdir out --gather
+      --ckptpath panacea.ckpt model.params.conditioner_config.params.emb_models.0.params.bpe_path=bpe_simple_vocab_16e6.txt.gz
 """
 from __future__ import annotations
 
@@ -65,9 +69,25 @@ def load_config(paths, overrides=()):
         node = cfg
         parts = k.split(".")
         for part in parts[:-1]:
-            node = node.setdefault(part, {})
-        node[parts[-1]] = yaml.safe_load(v)
+            node = _child(node, part, k)
+        if isinstance(node, list):
+            node[_list_index(node, parts[-1], k)] = yaml.safe_load(v)
+        else:
+            node[parts[-1]] = yaml.safe_load(v)
     return cfg
+
+
+def _list_index(node: list, part: str, key: str) -> int:
+    """A numeric path component indexes an existing list entry (emb_models.0.params...)."""
+    if not part.isdigit() or int(part) >= len(node):
+        raise KeyError(f"override {key!r}: {part!r} does not index the {len(node)}-entry list here")
+    return int(part)
+
+
+def _child(node, part: str, key: str):
+    if isinstance(node, list):
+        return node[_list_index(node, part, key)]
+    return node.setdefault(part, {})
 
 
 def _merge(a, b):

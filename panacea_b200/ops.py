@@ -213,13 +213,15 @@ class NativeOps:
         self.launches += 1
         return y
 
-    def layernorm(self, x, gamma, beta, eps=1e-5):
+    def layernorm(self, x, gamma, beta, eps=1e-5, out_f32=False):
+        """x [..., C] -> operand of the same shape (fp32 when out_f32: a final LayerNorm whose output leaves the network)."""
         _req(x.is_cuda and x.dtype in (F32, BF16) and x.is_contiguous(), "layernorm: x must be contiguous CUDA fp32 / bf16")
         Cc = x.shape[-1]
         rows = x.numel() // Cc
-        y = self._operand_empty(x.shape, x.device)
+        mode = OP_F32 if out_f32 else self.operand_mode
+        y = self._operand_empty(x.shape, x.device, mode)
         _lib.check(self.lib.pn_layernorm(_ptr(x), int(x.dtype == BF16), _ptr(gamma), _ptr(beta), _ptr(y), rows, Cc, float(eps),
-                                         self.operand_mode, _stream()), "pn_layernorm")
+                                         mode, _stream()), "pn_layernorm")
         self.launches += 1
         return y
 
@@ -280,6 +282,45 @@ class NativeOps:
         base = qkv.data_ptr()
         _lib.check(self.lib.pn_attention_temporal(base, base + 2 * Cc, base + 4 * Cc, out.data_ptr(), b, T, P, heads, d, C3, Cc,
                                                  d ** -0.5, _stream()), "pn_attention_temporal")
+        self.launches += 1
+        return out
+
+    def attention_causal(self, qkv, heads):
+        """qkv bf16 [b, L, 3C] (fused q|k|v channels, L <= 128) -> bf16 [b, L, C]; token i attends keys j <= i."""
+        _req(qkv.is_cuda and qkv.dtype == BF16 and qkv.is_contiguous() and qkv.dim() == 3, "attention_causal: qkv bf16 [b,L,3C]")
+        b, L, C3 = qkv.shape
+        Cc = C3 // 3
+        _req(Cc == heads * 64 and 1 <= L <= 128, "attention_causal: needs head_dim 64 and L <= 128")
+        out = torch.empty((b, L, Cc), device=qkv.device, dtype=BF16)
+        base = qkv.data_ptr()
+        _lib.check(self.lib.pn_attention_causal(base, base + 2 * Cc, base + 4 * Cc, out.data_ptr(), b, L, heads, 64, C3, Cc,
+                                               64 ** -0.5, _stream()), "pn_attention_causal")
+        self.launches += 1
+        return out
+
+    # ------------------------------------------------------------------ text encoder helpers
+    def gelu_operand(self, x):
+        """fp32 [..., C] -> GEMM operand of gelu_erf(x) (bf16; [..., 3C] split3 in parity mode)."""
+        _req(x.is_cuda and x.dtype == F32 and x.is_contiguous(), "gelu_operand: x must be contiguous CUDA fp32")
+        Cc = x.shape[-1]
+        y = self._operand_empty(x.shape, x.device)
+        _lib.check(self.lib.pn_gelu_operand(_ptr(x), _ptr(y), x.numel() // Cc, Cc, self.operand_mode, _stream()), "pn_gelu_operand")
+        self.launches += 1
+        return y
+
+    def token_embedding(self, tokens, table, pos):
+        """tokens int64 [b, L], table fp32 [vocab, width], pos fp32 [>= L, width] -> fp32 [b, L, width]."""
+        _req(tokens.is_cuda and tokens.dtype == torch.int64 and tokens.is_contiguous() and tokens.dim() == 2,
+             "token_embedding: tokens must be contiguous CUDA int64 [b, L]")
+        b, L = tokens.shape
+        vocab, width = table.shape
+        _req(table.dtype == F32 and table.is_contiguous() and pos.dtype == F32 and pos.is_contiguous() and pos.dim() == 2
+             and pos.shape[0] >= L and pos.shape[1] == width, "token_embedding: table fp32 [vocab, width], pos fp32 [L, width]")
+        lo, hi = int(tokens.min()), int(tokens.max())       # ids come from outside the program: checked before the launch
+        _req(0 <= lo and hi < vocab, f"token_embedding: token ids must lie in [0, {vocab}), got [{lo}, {hi}]")
+        out = torch.empty((b, L, width), device=tokens.device, dtype=F32)
+        _lib.check(self.lib.pn_token_embedding(_ptr(tokens), _ptr(table), _ptr(pos), _ptr(out), b, L, vocab, width, _stream()),
+                   "pn_token_embedding")
         self.launches += 1
         return out
 
@@ -540,5 +581,17 @@ class ParityOps(NativeOps):
         base = qkv.data_ptr()
         _lib.check(self.lib.pn_attention_temporal_f32(base, base + 4 * Cc, base + 8 * Cc, out.data_ptr(), b, T, P, heads, d, C3, d ** -0.5,
                                                      self.operand_mode, _stream()), "pn_attention_temporal_f32")
+        self.launches += 1
+        return out
+
+    def attention_causal(self, qkv, heads):
+        _req(qkv.is_cuda and qkv.dtype == F32 and qkv.is_contiguous() and qkv.dim() == 3, "attention_causal(parity): qkv fp32 [b,L,3C]")
+        b, L, C3 = qkv.shape
+        Cc = C3 // 3
+        _req(Cc == heads * 64 and 1 <= L <= 128, "attention_causal: needs head_dim 64 and L <= 128")
+        out = self._operand_empty((b, L, Cc), qkv.device)
+        base = qkv.data_ptr()
+        _lib.check(self.lib.pn_attention_causal_f32(base, base + 4 * Cc, base + 8 * Cc, out.data_ptr(), b, L, heads, 64, C3, 64 ** -0.5,
+                                                   self.operand_mode, _stream()), "pn_attention_causal_f32")
         self.launches += 1
         return out

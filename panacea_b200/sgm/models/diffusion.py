@@ -10,7 +10,7 @@ import torch.nn as nn
 
 from ..modules.diffusionmodules.sampling import BoundDenoiser
 from ..modules.diffusionmodules.wrappers import OpenAIWrapperControlLDM3D
-from ..modules.encoders.modules import VAEEmbedder
+from ..modules.encoders.modules import FrozenOpenCLIPEmbedder, VAEEmbedder
 from ..util import default, instantiate_from_config
 
 UNCONDITIONAL_CONFIG = {"target": "sgm.modules.GeneralConditioner", "params": {"emb_models": []}}
@@ -49,6 +49,8 @@ class DiffusionEngine3D(nn.Module):
         self.scale_factor = scale_factor
         self.disable_first_stage_autocast = disable_first_stage_autocast
         for emb in self.conditioner.embedders:                                     # diffusion.py:111-122 setup_vaeembedder
+            if precision is not None and isinstance(emb, FrozenOpenCLIPEmbedder):
+                emb.set_precision(precision)
             if isinstance(emb, VAEEmbedder):
                 emb.first_stage_model = self.first_stage_model
                 emb.disable_first_stage_autocast = disable_first_stage_autocast

@@ -2,15 +2,16 @@
 (reference sgm/modules/encoders/modules.py:95-220) with the three embedders configs/inference_nuscenes.yaml:73-93 names.
 
 The conditioner runs ONCE per sample, before the denoising loop; it only routes tensors (rearrange, cat, zeros for the
-unconditional branch) and is therefore plain host/torch code, like the reference's. The learned embedders are OUT OF
-SCOPE of this repository (BASELINE.json configs[3]: "random-init VAE/CLIP stubs"): `FrozenOpenCLIPEmbedder` here is a
-deterministic stand-in that maps each prompt string to a reproducible [77, 1024] tensor — there are no OpenCLIP weights in
-this environment — and `VAEEmbedder` delegates to whatever first-stage model the engine hands it (a stub or a real one).
+unconditional branch) and is therefore plain host/torch code, like the reference's. `FrozenOpenCLIPEmbedder` runs the
+OpenCLIP ViT-H/14 text tower on the sm_90a kernels (panacea_b200.text_encoder) once text-tower weights are loaded;
+without them it stays a deterministic stand-in that maps each prompt string to a reproducible [77, context_dim] tensor.
+`VAEEmbedder` delegates to whatever first-stage model the engine hands it (the native VAE).
 """
 from __future__ import annotations
 
 import hashlib
 from contextlib import nullcontext
+from pathlib import Path
 
 import torch
 import torch.nn as nn
@@ -40,28 +41,164 @@ class IdentityEncoder(AbstractEmbModel):
 
 
 class FrozenOpenCLIPEmbedder(AbstractEmbModel):
-    """Stand-in for modules.py:555-640 (OpenCLIP ViT-H/14 text tower, penultimate layer, [b, 77, 1024]). The real tower
-    and its weights are not available here and are outside the hot path; this stub keeps the interface and is
-    deterministic per prompt string, so the conditional ("a driving scene ...") and unconditional ("") branches differ
-    reproducibly on every rank."""
+    """modules.py:559-632: the OpenCLIP ViT-H/14 text tower, [b, 77, 1024] from the penultimate (or last) block.
+
+    With text-tower weights the tower runs natively (`panacea_b200.text_encoder.TextEncoderEngine`, sm_90a kernels, no
+    CPU path). Weights come from `version=<local open_clip file>` (.bin / .pt / .safetensors; `visual.*` ignored; a
+    pretrained tag such as the default loads nothing) or from a state dict with `<prefix>model.*` keys, e.g. an engine
+    checkpoint's `conditioner.embedders.0.model.*`. They appear in `state_dict()` under the same names. `forward` takes
+    prompt strings (tokenized with the CLIP BPE vocabulary from `bpe_path=`, else open_clip's bundled copy) or an int64
+    [b, 77] token tensor. `precision` ("bf16" | "parity", default env PN_PRECISION) selects the op set, as on the UNet.
+
+    Without weights it is a deterministic stand-in: each prompt string maps to a reproducible randn [77, context_dim],
+    so the conditional and unconditional ("") branches differ reproducibly on every rank."""
+    LAYERS = ("last", "penultimate")
+    FILE_SUFFIXES = (".bin", ".pt", ".pth", ".safetensors")
 
     def __init__(self, arch="ViT-H-14", version="laion2b_s32b_b79k", device="cuda", max_length=77, freeze=True,
-                 layer="penultimate", always_return_pooled=False, legacy=True, context_dim=1024):
+                 layer="penultimate", always_return_pooled=False, legacy=True, context_dim=1024, bpe_path=None,
+                 precision=None):
         super().__init__()
+        if layer not in self.LAYERS:
+            raise ValueError(f"layer must be one of {self.LAYERS}, got {layer!r}")
         self.max_length, self.context_dim = max_length, context_dim
+        self.layer_idx = 1 if layer == "penultimate" else 0
+        self.bpe_path = bpe_path
         self.register_buffer("_dev", torch.zeros(1), persistent=False)
+        self._tower_keys = []                  # open_clip names of the loaded tower tensors (buffers "t__<name>")
+        self._tokenizer = None
+        self._engine = None
+        self._version, self._packed = 0, -1
+        self.set_precision(precision)
+        if isinstance(version, str) and version.endswith(self.FILE_SUFFIXES):
+            self._set_tower(_read_open_clip_file(version), source=version)
+
+    # --- weights
+    def set_precision(self, precision) -> None:
+        """"bf16" or "parity"; the tower is repacked on the next call."""
+        from ..diffusionmodules.controlmodel import _resolve_precision
+        self.precision = _resolve_precision(precision)
+        self._engine = None
+
+    @property
+    def has_tower(self) -> bool:
+        return bool(self._tower_keys)
+
+    def _tower_errors(self, sd: dict) -> list:
+        from ....text_encoder import text_config_from_params, text_param_spec
+        if "token_embedding.weight" not in sd or "positional_embedding" not in sd:
+            return ["missing " + ", ".join(k for k in ("token_embedding.weight", "positional_embedding") if k not in sd)]
+        cfg = text_config_from_params(sd)
+        spec = text_param_spec(**cfg)
+        missing = [k for k in spec if k not in sd]
+        if missing:
+            return [f"missing {len(missing)} keys: {', '.join(missing[:12])}{' ...' if len(missing) > 12 else ''}"]
+        bad = [k for k, s in spec.items() if tuple(sd[k].shape) != s]
+        if bad:
+            return [f"misshaped: {', '.join(f'{k} {tuple(sd[k].shape)}' for k in bad[:6])}"]
+        errs = []
+        if cfg["width"] != self.context_dim:
+            errs.append(f"tower width {cfg['width']} != context_dim {self.context_dim}")
+        if cfg["ctx"] != self.max_length:
+            errs.append(f"positional_embedding has {cfg['ctx']} positions, max_length is {self.max_length}")
+        if cfg["width"] % 64:
+            errs.append(f"tower width {cfg['width']} is not a multiple of head_dim 64")
+        if cfg["layers"] <= self.layer_idx:
+            errs.append(f"{cfg['layers']} blocks cannot serve layer_idx {self.layer_idx}")
+        return errs
+
+    def _set_tower(self, sd: dict, source: str) -> None:
+        sd = {k: v for k, v in sd.items() if not k.startswith("visual.")}
+        errs = self._tower_errors(sd)
+        if errs:
+            raise ValueError(f"FrozenOpenCLIPEmbedder: text tower from {source}: " + "; ".join(errs))
+        for k in self._tower_keys:
+            delattr(self, "t__" + k.replace(".", "__"))
+        self._tower_keys = sorted(sd)
+        for k in self._tower_keys:
+            self.register_buffer("t__" + k.replace(".", "__"), sd[k].detach().clone().to(self._dev.device), persistent=False)
+        self._version += 1
+
+    def tower_parameters(self) -> dict:
+        return {k: getattr(self, "t__" + k.replace(".", "__")) for k in self._tower_keys}
+
+    def _save_to_state_dict(self, destination, prefix, keep_vars):
+        for k, v in self.tower_parameters().items():
+            destination[prefix + "model." + k] = v
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs):
+        p = prefix + "model."
+        sd = {k[len(p):]: v for k, v in state_dict.items() if k.startswith(p)}
+        if not sd:
+            return                              # no tower in this state dict: the embedder keeps what it has
+        sd = {k: v for k, v in sd.items() if not k.startswith("visual.")}
+        errs = self._tower_errors(sd)
+        if errs:
+            error_msgs.append(f"text tower under {p}*: " + "; ".join(errs))
+            return
+        self._set_tower(sd, source=p + "*")
+
+    def _apply(self, fn, recurse=True):
+        r = super()._apply(fn, recurse)
+        self._version += 1
+        return r
+
+    # --- forward
+    def tokenize(self, text) -> torch.Tensor:
+        if self._tokenizer is None:
+            from ....clip_tokenizer import ClipTokenizer
+            self._tokenizer = ClipTokenizer(self.bpe_path)
+        return self._tokenizer.tokenize(list(text), self.max_length)
+
+    def engine(self):
+        from ....text_encoder import TextEncoderEngine
+        if self._engine is None:
+            from ..diffusionmodules.controlmodel import _native_ops
+            self._engine = TextEncoderEngine(_native_ops(self.precision))
+            self._packed = -1
+        if self._packed != self._version:
+            self._engine.pack(self.tower_parameters())
+            self._packed = self._version
+        return self._engine
 
     def encode(self, text):
         return self(text)
 
     @torch.no_grad()
     def forward(self, text):
+        if not self.has_tower:
+            return self._stand_in(text)
+        dev = self._dev.device
+        if dev.type != "cuda":
+            raise RuntimeError("panacea_b200 runs on CUDA (sm_90a) only; the text tower has no CPU path (call .cuda())")
+        if isinstance(text, torch.Tensor):
+            if text.dtype != torch.int64 or text.dim() != 2 or text.shape[1] != self.max_length:
+                raise ValueError(f"token tensor must be int64 [b, {self.max_length}], got {text.dtype} {tuple(text.shape)}")
+            tokens = text
+        else:
+            tokens = self.tokenize(text)
+        return self.engine().encode(tokens.to(dev), self.layer_idx)
+
+    def _stand_in(self, text):
         outs = []
         for s in text:
             seed = int.from_bytes(hashlib.sha256(str(s).encode()).digest()[:8], "little") % (2 ** 63)
             g = torch.Generator().manual_seed(seed)
             outs.append(torch.randn(self.max_length, self.context_dim, generator=g))
         return torch.stack(outs).to(self._dev.device)
+
+
+def _read_open_clip_file(path: str) -> dict:
+    """A stock open_clip weights file (the reference's commented-out local-file alternative, modules.py:580-583)."""
+    if not Path(path).is_file():
+        raise FileNotFoundError(f"FrozenOpenCLIPEmbedder: version={path!r} names a weights file that does not exist")
+    if path.endswith(".safetensors"):
+        from safetensors.torch import load_file
+        sd = load_file(path)
+    else:
+        sd = torch.load(path, map_location="cpu", weights_only=True)
+        sd = sd.get("state_dict", sd)
+    return {k[len("module."):] if k.startswith("module.") else k: v for k, v in sd.items()}
 
 
 class VAEEmbedder(AbstractEmbModel):

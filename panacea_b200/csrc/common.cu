@@ -182,7 +182,7 @@ bool pdl_enabled() {
   return on;
 }
 
-int ensure_dyn_smem(const void* func, size_t bytes) {
+int ensure_dyn_smem(const void* func, size_t bytes, bool max_carveout) {
   int dev = 0;
   cudaGetDevice(&dev);
   const unsigned long long key = (unsigned long long)reinterpret_cast<uintptr_t>(func) ^ ((unsigned long long)(dev & 0xff) << 56);
@@ -190,6 +190,8 @@ int ensure_dyn_smem(const void* func, size_t bytes) {
   auto it = g_smem_attr.find(key);
   if (it != g_smem_attr.end() && it->second >= bytes) return PN_OK;
   PN_CHECK_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  if (max_carveout)
+    PN_CHECK_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
   g_smem_attr[key] = bytes;
   return PN_OK;
 }

@@ -41,8 +41,9 @@ int cached_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_
                      const uint64_t* strides_elems, const uint32_t* box, int swizzle_bytes);
 
 int sm_count();                                          // of the current device
-// opt in to `bytes` of dynamic shared memory for `func` on the current device (once per device and size)
-int ensure_dyn_smem(const void* func, size_t bytes);
+// opt in to `bytes` of dynamic shared memory for `func` on the current device (once per device and size);
+// `max_carveout` also asks for the largest shared-memory carveout, for kernels that plan on several CTAs per SM
+int ensure_dyn_smem(const void* func, size_t bytes, bool max_carveout = false);
 
 // PN_PDL=1 enables programmatic dependent launch (off by default: measured no gain on the captured graph)
 bool pdl_enabled();

@@ -9,11 +9,17 @@
 // 455-462 Conv2d(padding=1) on the width-concatenated 6-view image; :418,468-476 Conv1d(k=3,padding=1)).
 // B is the packed weight matrix [N, taps*C] (K-major, bf16). Accumulation is fp32 in registers.
 //
-// Kernel structure (one CTA per 128 x BN output tile, 288 threads):
+// Kernel structure (one CTA per 128 x BN output tile, 256 threads, TWO CTAs per SM):
 //   warps 0-3, 4-7 : two consumer warpgroups, 64 tile rows each: wgmma m64nBNk16 from the shared-memory ring,
 //                    then the epilogue straight from the accumulator registers (bias / row vector / LayerNorm fold /
 //                    GEGLU / residuals -> global)
-//   warp 8         : TMA producer (A box [tn,th,tw,64] + B box [BN,64] per k-block, 128B swizzle)
+//   thread 0       : also issues the TMA loads (A box [tn,th,tw,64] + B box [BN,64] per k-block, 128B swizzle): the
+//                    first STAGES - 1 k-blocks up front, then one per k-block from inside the consumer loop, into the
+//                    stage both warpgroups have just released.
+// Two co-resident CTAs per SM let one tile's barrier set-up, first load latency and epilogue run under the other
+// tile's MMAs. That needs <= 4 warps per SM sub-partition (a 9-warp CTA with a dedicated producer warp puts 5 warps on
+// one sub-partition for two CTAs, capping threads at 96 registers, below the 80-float m64n160 accumulator plus
+// addressing) and <= 114 KB of shared memory per CTA (3 stages at BN = 160).
 // Pipeline: STAGES-deep full/empty mbarrier ring; a stage is handed back once the wgmma group that read it retired.
 #include "common.cuh"
 #include "ptx.cuh"
@@ -23,7 +29,10 @@ namespace pn {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle atom row
-constexpr int GEMM_THREADS = 288;
+constexpr int SM_SMEM_BYTES = 233472;      // 228 KB of shared memory per H100 SM ...
+constexpr int CTA_SMEM_RESERVED = 1024;    // ... of which the system reserves 1 KB per resident CTA
+constexpr int GEMM_THREADS = 256;
+constexpr int GEMM_CTAS_PER_SM = 2;
 
 struct GemmParams {
   CUtensorMap mapA;
@@ -68,7 +77,7 @@ struct GemmSmem {
 // MODE: 0 = fp32 store (+ fp32 residual, + second fp32 residual), 1 = bf16 store (+ fp32 or bf16 residual, LayerNorm
 // fold / row statistics), 2 = GEGLU (bf16 store of N/2 columns)
 template <int BN, int STAGES, int MODE>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
+__global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   using S = GemmSmem<BN, STAGES>;
   constexpr int NJ = BN / 8;                   // 8-column accumulator blocks per thread row
   extern __shared__ uint8_t smem_raw[];
@@ -98,29 +107,20 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   __syncthreads();
   pdl_prologue_done();        // barriers are set up: from here on global memory is touched
 
-  if (warp == 8) {
-    // ===================== TMA producer (warp-wide loop, TMA issue under elect.sync) =====================
-    const int x0 = twi * p.tw, y0 = thi * p.th, n0 = tni * p.tn;
-    const int bn0 = tcol * BN;
-    int stage = 0;
-    uint32_t phase = 0;
-    int kc = 0, dx = -p.pad_w, dy = -p.pad_h;   // k-block -> (tap row, tap column, channel chunk), kept incrementally
-    for (int kb = 0; kb < num_k_blocks; ++kb) {
-      mbar_wait(&empty_bar[stage], phase ^ 1);
-      if (elect_one()) {
-        uint8_t* sA = smem + stage * S::STAGE_BYTES;
-        mbar_arrive_expect_tx(&full_bar[stage], S::STAGE_BYTES);
-        tma_load_4d(sA, &p.mapA, &full_bar[stage], kc * BK, x0 + dx, y0 + dy, n0);
-        tma_load_2d(sA + S::A_BYTES, &p.mapB, &full_bar[stage], kb * BK, bn0);
-      }
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      if (++kc == p.kc_per_tap) {
-        kc = 0;
-        if (++dx > p.taps_w - 1 - p.pad_w) { dx = -p.pad_w; ++dy; }
-      }
+  // The next k-block to load -> (tap row, tap column, 64-channel chunk), channel chunk fastest, advanced one k-block at
+  // a time. Every thread keeps it, so thread 0's loads are issued by predicate, not by branch.
+  int ld_kb = 0, ld_kc = 0, ld_dx = -p.pad_w, ld_dy = -p.pad_h;
+  auto load_next = [&](int stage, bool issue) {
+    uint8_t* sA = smem + stage * S::STAGE_BYTES;
+    tma_load_stage_if(issue, &full_bar[stage], S::STAGE_BYTES, sA, &p.mapA, ld_kc * BK, twi * p.tw + ld_dx, thi * p.th + ld_dy,
+                      tni * p.tn, sA + S::A_BYTES, &p.mapB, ld_kb * BK, tcol * BN);
+    ++ld_kb;
+    if (++ld_kc == p.kc_per_tap) {
+      ld_kc = 0;
+      if (++ld_dx > p.taps_w - 1 - p.pad_w) { ld_dx = -p.pad_w; ++ld_dy; }
     }
-    return;
-  }
+  };
+  for (int s = 0; s < STAGES - 1 && s < num_k_blocks; ++s) load_next(s, threadIdx.x == 0);
 
   // ===================== consumer warpgroups =====================
   const int wg = warp >> 2;
@@ -132,8 +132,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     const uint64_t descA0 = wgmma_desc(base + wg * (64 * 128), 16, 1024, kSw128);
     const uint64_t descB0 = wgmma_desc(base + S::A_BYTES, 16, 1024, kSw128);
     constexpr uint64_t STAGE_STEP = S::STAGE_BYTES >> 4;      // start-address field is in 16-byte units
-    int stage = 0, prev = 0;
-    uint32_t phase = 0;
+    // prev = the stage of k-block kb - 1 = the stage k-block kb + STAGES - 1 is loaded into. Before the first k-block
+    // it is the last, still unused stage: its empty barrier's "previous" phase (parity 1) counts as complete.
+    int stage = 0, prev = STAGES - 1;
+    uint32_t phase = 0, prev_phase = 1;
     for (int kb = 0; kb < num_k_blocks; ++kb) {
       mbar_wait(&full_bar[stage], phase);
       wgmma_fence();
@@ -143,7 +145,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       wgmma_commit();
       wgmma_wait<1>();                         // the group of the previous k-block has retired: refill its stage
       if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      // Once BOTH warpgroups have released the stage (the empty barrier's phase for that use completes), thread 0 loads
+      // k-block kb + STAGES - 1 into it. Every consumer thread waits and the load is predicated: a branch that depends
+      // on the thread (or a conditional wait) while this k-block's wgmma group is in flight makes ptxas serialise the
+      // wgmma instructions (C7518 / C7515).
+      mbar_wait(&empty_bar[prev], prev_phase);
+      load_next(prev, threadIdx.x == 0 && kb + STAGES - 1 < num_k_blocks);
       prev = stage;
+      prev_phase = phase;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
     wgmma_wait<0>();
@@ -287,10 +296,11 @@ static void pick_tile(long long NB, long long H, long long W, int* tw, int* th, 
 template <int BN, int STAGES>
 static int launch_gemm(const GemmParams& p, int mode, long long tiles, cudaStream_t stream) {
   using S = GemmSmem<BN, STAGES>;
-  static_assert(S::TOTAL <= 232448, "shared memory budget exceeded (227 KB per block)");
+  static_assert(GEMM_CTAS_PER_SM * (S::TOTAL + CTA_SMEM_RESERVED) <= SM_SMEM_BYTES,
+                "shared memory budget exceeded: two CTAs must fit one SM");
   void (*kern)(GemmParams) = mode == 2 ? gemm_tc_kernel<BN, STAGES, 2> : mode == 1 ? gemm_tc_kernel<BN, STAGES, 1>
                                                                                    : gemm_tc_kernel<BN, STAGES, 0>;
-  const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), S::TOTAL);
+  const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), S::TOTAL, /*max_carveout=*/true);
   if (rc != PN_OK) return rc;
   PN_CHECK_CUDA(launch_kernel(kern, dim3((unsigned)tiles), dim3(GEMM_THREADS), S::TOTAL, stream, 1, p));
   return PN_OK;
@@ -381,10 +391,11 @@ extern "C" int pn_gemm(const pn_gemm_args* a, void* stream_v) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   const int mode = a->geglu ? 2 : a->out_bf16 ? 1 : 0;
   switch (BN) {
-    case 160: return launch_gemm<160, 5>(p, mode, tiles, stream);
-    case 128: return launch_gemm<128, 6>(p, mode, tiles, stream);
-    case 64: return launch_gemm<64, 8>(p, mode, tiles, stream);
-    default: return launch_gemm<32, 8>(p, mode, tiles, stream);
+    // the deepest rings that still fit two CTAs per SM (111,664 / 99,376 / 99,392 / 103,504 bytes per CTA)
+    case 160: return launch_gemm<160, 3>(p, mode, tiles, stream);
+    case 128: return launch_gemm<128, 3>(p, mode, tiles, stream);
+    case 64: return launch_gemm<64, 4>(p, mode, tiles, stream);
+    default: return launch_gemm<32, 5>(p, mode, tiles, stream);
   }
 }
 

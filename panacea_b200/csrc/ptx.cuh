@@ -108,6 +108,24 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// One ring stage of a GEMM: expect_tx of `bytes` on `bar`, then a 4-D A box and a 2-D B box completing on it, issued
+// only where `pred` holds. Predicated instructions rather than a branch: a thread-divergent branch between wgmma issue
+// and wait makes ptxas serialise the wgmma instructions (C7518).
+__device__ __forceinline__ void tma_load_stage_if(bool pred, uint64_t* bar, uint32_t bytes, void* dst_a, const CUtensorMap* map_a,
+                                                  int a0, int a1, int a2, int a3, void* dst_b, const CUtensorMap* map_b, int b0,
+                                                  int b1) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %0, 0;\n"
+      "@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%1], %2;\n"
+      "@p cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%3], [%4, {%5, %6, %7, %8}], [%1];\n"
+      "@p cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%9], [%10, {%11, %12}], [%1];\n"
+      "}\n"
+      ::"r"((uint32_t)pred), "r"(smem_u32(bar)), "r"(bytes), "r"(smem_u32(dst_a)), "l"(reinterpret_cast<uint64_t>(map_a)),
+      "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(smem_u32(dst_b)), "l"(reinterpret_cast<uint64_t>(map_b)), "r"(b0), "r"(b1)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
                                             int c2, int c3, int c4) {
   asm volatile(

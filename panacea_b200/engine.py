@@ -475,11 +475,10 @@ class Engine:
         if self.two_streams and xin.is_cuda:
             # The ControlNet and the UNet's own encoder + middle block only meet at the first skip join (controlmodel.py:
             # 176-195): they run on two streams (a fork / join pair of events, captured into the step's CUDA graph like
-            # everything else). The big level-0/1 kernels are persistent and fill all SMs either way; what overlaps is
-            # the under-filled tail — level-2/3/mid GEMMs and attentions with fewer tiles than SMs, small norms:
-            # 112.4 -> 111.1 ms per step on the same box (PN_TWO_STREAMS=0 for the single-stream order). Giving each branch
-            # a fixed share of the SMs (74/100/120 per branch) instead of letting the kernels queue was measured and is not
-            # better (112.3 / 115.5 / 113.7 ms).
+            # everything else). The big level-0/1 launches have many waves of tiles and fill all SMs either way; what
+            # overlaps is the under-filled tail — level-2/3/mid GEMMs and attentions with fewer tiles than SMs, small
+            # norms — and, since the GEMM kernel fits two CTAs per SM, a GEMM tile of one branch can share an SM with a
+            # tile of the other. PN_TWO_STREAMS=0 restores the single-stream order.
             cur = torch.cuda.current_stream(xin.device)
             if self._side is None or self._side.device != xin.device:
                 self._side = torch.cuda.Stream(device=xin.device)

@@ -40,8 +40,11 @@ enum pn_status { PN_STATUS_OK = 0, PN_STATUS_INVALID = -1, PN_STATUS_CUDA = -2, 
  *                    packed [W_hi | W_hi | W_lo] per tap the same pn_gemm kernel yields fp32-class products
  *                    (hi W_hi + lo W_hi + hi W_lo), which is how the reference's fp32 math (wrappers.py:37-70 on CPU)
  *                    is matched to rtol 1e-3 / atol 1e-4;
- *  PN_OPERAND_F32    fp32 [rows, C]                   — input of a CUDA-core consumer in parity mode. */
-enum pn_operand_mode { PN_OPERAND_BF16 = 0, PN_OPERAND_SPLIT3 = 1, PN_OPERAND_F32 = 2 };
+ *  PN_OPERAND_F32    fp32 [rows, C]                   — input of a CUDA-core consumer in parity mode;
+ *  PN_OPERAND_SPLIT3_B bf16 [rows, 3C] = [hi | hi | lo] — the WEIGHT form (the layout ops.split3 packs weights in), made
+ *                    on the device for a GEMM whose B factor is an activation (the VAE mid-block attention's k and v).
+ *                    Only pn_cast_operand accepts it; every other entry point with an operand_mode rejects it. */
+enum pn_operand_mode { PN_OPERAND_BF16 = 0, PN_OPERAND_SPLIT3 = 1, PN_OPERAND_F32 = 2, PN_OPERAND_SPLIT3_B = 3 };
 
 const char* pn_last_error(void);
 int pn_abi_version(void);
@@ -153,6 +156,10 @@ int pn_attention_causal_f32(const float* q, const float* k, const float* v, void
  * all six views of the panorama. raw_bf16 (optional) receives a plain bf16 cast of x (input of the 1x1 skip
  * convolution, openaimodel.py:486). workspace: pn_groupnorm_workspace_floats(...) floats. */
 int64_t pn_groupnorm_workspace_floats(int64_t frames, int64_t pixels, int64_t channels);
+/* How many pixel ranges pn_groupnorm_silu splits each frame's statistics into for a call of this shape. Each frame's
+ * result depends on the frame count only through this number, so calls over subsets of the frames that give the same
+ * value reproduce one call over all of them bit for bit (the VAE's frame chunking checks it). */
+int64_t pn_groupnorm_ctas_per_frame(int64_t frames, int64_t pixels, int64_t channels);
 int pn_groupnorm_silu(const float* x, const float* gamma, const float* beta, void* y, void* raw,
                       float* workspace, int64_t frames, int64_t pixels, int64_t channels, float eps, int act_silu,
                       int operand_mode, void* stream);
@@ -185,7 +192,7 @@ int pn_upsample2x(const float* x, void* y, int64_t frames, int64_t H, int64_t W,
 int pn_concat_add(const float* h, const float* skip, const float* ctrl, float* out, int64_t rows, int64_t C1,
                   int64_t C2, void* stream);
 int pn_add_inplace(float* x, const float* y, int64_t n, void* stream);      /* h += control.pop() (controlmodel.py:192) */
-/* fp32 [rows, C] -> operand (bf16 or split3). */
+/* fp32 [rows, C] -> operand: bf16, split3 A form [hi | lo | hi] or split3 weight form [hi | hi | lo] (operand_mode 0, 1, 3). */
 int pn_cast_operand(const float* x, void* y, int64_t rows, int64_t C, int operand_mode, void* stream);
 /* Parity-mode GEGLU (attention.py:97-99, exact erf GELU) on the fp32 output of the ff.net.0 GEMM whose columns are in
  * pn_gemm's GEGLU packing (blocks of 32 = 16 value + 16 gate columns): in fp32 [rows, 2*inner] -> operand [rows, inner]. */
@@ -212,6 +219,11 @@ int pn_linear_small(const float* x, const void* W, int w_is_f32, const float* bi
  * single-head attention of the VAE mid block (reference sgm/modules/diffusionmodules/model.py:374-414, head_dim = C). */
 int pn_softmax_rows(const float* in, void* out_bf16, int64_t rows, int64_t N, int64_t ld_in, int64_t ld_out, float scale,
                     void* stream);
+/* pn_softmax_rows storing the probabilities as the A operand of the O = P v GEMM: operand_mode PN_OPERAND_BF16 (bitwise
+ * the output of pn_softmax_rows) or PN_OPERAND_SPLIT3 (out bf16 [rows, 3N] = [hi | lo | hi], parity mode). ld_out counts
+ * bf16 elements (>= 3N for split3). N <= 51,200 (the row is staged in shared memory), N % 4 == 0. */
+int pn_softmax_rows_operand(const float* in, void* out, int64_t rows, int64_t N, int64_t ld_in, int64_t ld_out, float scale,
+                            int operand_mode, void* stream);
 /* Content fingerprint of a device buffer (two order-independent 64-bit sums over its 32-bit words) -> out2[2] on the
  * device. The wrapper keys its step-invariant conditioning cache (BEV hint stem, text K/V; wrappers.py:37-70 recomputes
  * them every step) on the CONTENT of c["cond_feat"] / c["crossattn"]: addresses are recycled by the allocator. */

@@ -73,6 +73,7 @@ SIGNATURES: dict[str, tuple] = {
     "pn_attention_causal": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i64, _i64, _f32, _vp]),
     "pn_attention_causal_f32": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i64, _f32, C.c_int, _vp]),
     "pn_groupnorm_workspace_floats": (_i64, [_i64, _i64, _i64]),
+    "pn_groupnorm_ctas_per_frame": (_i64, [_i64, _i64, _i64]),
     "pn_groupnorm_silu": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _f32, C.c_int, C.c_int, _vp]),
     "pn_groupnorm_pixel_silu": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _f32, C.c_int, C.c_int, _vp]),
     "pn_layernorm": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp, _i64, _i64, _f32, C.c_int, _vp]),
@@ -94,6 +95,7 @@ SIGNATURES: dict[str, tuple] = {
     "pn_scale_dup": (C.c_int, [_vp, _vp, _i64, _f32, C.c_int, _vp]),
     "pn_fingerprint": (C.c_int, [_vp, _i64, _vp, _vp]),
     "pn_softmax_rows": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _f32, _vp]),
+    "pn_softmax_rows_operand": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _f32, C.c_int, _vp]),
 }
 
 

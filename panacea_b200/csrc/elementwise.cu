@@ -278,10 +278,13 @@ __global__ void scale_dup_kernel(const float* __restrict__ x, float* __restrict_
   }
 }
 
-// ---------------------------------------------------------------- row softmax, fp32 scores -> bf16 probabilities
+// ---------------------------------------------------------------- row softmax, fp32 scores -> GEMM operand
 // The single-head, C-wide attention of the VAE mid block (reference model.py:374-414: SDPA over all h*w tokens with
-// head_dim = C = 512) is run as GEMMs (S = q k^T, O = P v) around this kernel: out[r, :] = softmax(scale * in[r, :]).
-// One CTA per row; the row's exponentials are kept in shared memory between the sum and the normalised store.
+// head_dim = C = 512) is run as GEMMs (S = q k^T, O = P v) around this kernel: out[r, :] = softmax(scale * in[r, :]),
+// stored as the A operand of the O GEMM: bf16 [rows, N] (OP = PN_OP_BF16) or split3 [rows, 3N] = [hi | lo | hi]
+// (OP = PN_OP_SPLIT3, parity mode). ld_out counts bf16 elements. One CTA per row; the row's exponentials are kept in
+// shared memory between the sum and the normalised store.
+template <int OP>
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ in, __nv_bfloat16* __restrict__ out, int N,
                                                            long long ld_in, long long ld_out, float scale_log2) {
   pdl_prologue_done();
@@ -323,7 +326,8 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
   const float inv = 1.f / s;
   for (int i = threadIdx.x * 4; i < N; i += 1024) {
     const float4 v = *reinterpret_cast<float4*>(sm_row + i);
-    *reinterpret_cast<uint2*>(dst + i) = make_uint2(pack_bf16x2(v.x * inv, v.y * inv), pack_bf16x2(v.z * inv, v.w * inv));
+    const float o[4] = {v.x * inv, v.y * inv, v.z * inv, v.w * inv};
+    store_op4<OP>(dst, 0, N, i, o);       // row 0 of a "matrix" starting at this row: split3 thirds at +N, +2N
   }
 }
 
@@ -403,10 +407,15 @@ extern "C" int pn_add_inplace(float* x, const float* y, int64_t n, void* stream_
 
 extern "C" int pn_cast_operand(const float* x, void* y, int64_t rows, int64_t C, int operand_mode, void* stream_v) {
   PN_REQUIRE(x && y && rows > 0 && C > 0 && C % 4 == 0, "pn_cast_operand: bad arguments");
-  PN_REQUIRE(operand_mode == PN_OP_BF16 || operand_mode == PN_OP_SPLIT3, "pn_cast_operand: operand_mode %d", operand_mode);
+  PN_REQUIRE(operand_mode == PN_OP_BF16 || operand_mode == PN_OP_SPLIT3 || operand_mode == PN_OP_SPLIT3_B,
+             "pn_cast_operand: operand_mode %d", operand_mode);
   const size_t n4 = (size_t)rows * (size_t)(C / 4);
-  PN_DISPATCH_OP(operand_mode, (launch_kernel(cast_operand_kernel<OP>, dim3(grid_for(n4)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream_v), 1, 
-      x, y, (size_t)rows, (int)C)));
+  if (operand_mode == PN_OP_SPLIT3_B)
+    launch_kernel(cast_operand_kernel<PN_OP_SPLIT3_B>, dim3(grid_for(n4)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream_v), 1,
+                  x, y, (size_t)rows, (int)C);
+  else
+    PN_DISPATCH_OP(operand_mode, (launch_kernel(cast_operand_kernel<OP>, dim3(grid_for(n4)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream_v), 1, 
+        x, y, (size_t)rows, (int)C)));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
@@ -507,17 +516,37 @@ extern "C" int pn_fingerprint(const void* x, int64_t nbytes, uint64_t* out2, voi
   return PN_OK;
 }
 
-extern "C" int pn_softmax_rows(const float* in, void* out_bf16, int64_t rows, int64_t N, int64_t ld_in, int64_t ld_out, float scale,
-                               void* stream_v) {
-  PN_REQUIRE(in && out_bf16 && rows > 0 && N > 0 && N % 4 == 0 && ld_in >= N && ld_out >= N && ld_in % 4 == 0 && ld_out % 4 == 0,
-             "pn_softmax_rows: bad arguments");
-  PN_REQUIRE(N * 4 <= 200 * 1024, "pn_softmax_rows: N=%lld exceeds the shared-memory row buffer", (long long)N);
-  PN_REQUIRE(rows < (1ll << 31), "pn_softmax_rows: too many rows");
+static int softmax_rows_launch(const float* in, void* out, int64_t rows, int64_t N, int64_t ld_in, int64_t ld_out, float scale,
+                               int operand_mode, void* stream_v, const char* who) {
+  const int64_t width = operand_mode == PN_OP_SPLIT3 ? 3 * N : N;
+  PN_REQUIRE(in && out && rows > 0 && N > 0 && N % 4 == 0 && ld_in >= N && ld_out >= width && ld_in % 4 == 0 && ld_out % 4 == 0,
+             "%s: bad arguments", who);
+  PN_REQUIRE(N * 4 <= 200 * 1024, "%s: N=%lld exceeds the shared-memory row buffer", who, (long long)N);
+  PN_REQUIRE(rows < (1ll << 31), "%s: too many rows", who);
   const size_t smem = (size_t)N * sizeof(float);
-  const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(&softmax_rows_kernel), smem);
-  if (rc != PN_OK) return rc;
-  launch_kernel(softmax_rows_kernel, dim3((unsigned)rows), dim3(256), smem, reinterpret_cast<cudaStream_t>(stream_v), 1, 
-      in, reinterpret_cast<__nv_bfloat16*>(out_bf16), (int)N, ld_in, ld_out, scale * 1.4426950408889634f);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+  const float scale_log2 = scale * 1.4426950408889634f;
+  __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
+  if (operand_mode == PN_OP_SPLIT3) {
+    const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(&softmax_rows_kernel<PN_OP_SPLIT3>), smem);
+    if (rc != PN_OK) return rc;
+    launch_kernel(softmax_rows_kernel<PN_OP_SPLIT3>, dim3((unsigned)rows), dim3(256), smem, st, 1, in, o, (int)N, ld_in, ld_out, scale_log2);
+  } else {
+    const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(&softmax_rows_kernel<PN_OP_BF16>), smem);
+    if (rc != PN_OK) return rc;
+    launch_kernel(softmax_rows_kernel<PN_OP_BF16>, dim3((unsigned)rows), dim3(256), smem, st, 1, in, o, (int)N, ld_in, ld_out, scale_log2);
+  }
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
+}
+
+extern "C" int pn_softmax_rows(const float* in, void* out_bf16, int64_t rows, int64_t N, int64_t ld_in, int64_t ld_out, float scale,
+                               void* stream_v) {
+  return softmax_rows_launch(in, out_bf16, rows, N, ld_in, ld_out, scale, PN_OP_BF16, stream_v, "pn_softmax_rows");
+}
+
+extern "C" int pn_softmax_rows_operand(const float* in, void* out, int64_t rows, int64_t N, int64_t ld_in, int64_t ld_out, float scale,
+                                       int operand_mode, void* stream_v) {
+  PN_REQUIRE(operand_mode == PN_OP_BF16 || operand_mode == PN_OP_SPLIT3, "pn_softmax_rows_operand: operand_mode %d", operand_mode);
+  return softmax_rows_launch(in, out, rows, N, ld_in, ld_out, scale, operand_mode, stream_v, "pn_softmax_rows_operand");
 }

@@ -403,6 +403,12 @@ extern "C" int64_t pn_groupnorm_workspace_floats(int64_t frames, int64_t pixels,
   return frames * cpf * GN_GROUPS * 2 + frames;      // partial sums + one arrival counter per frame
 }
 
+extern "C" int64_t pn_groupnorm_ctas_per_frame(int64_t frames, int64_t pixels, int64_t channels) {
+  int wave, cpf;
+  gn_geometry(frames, pixels, channels, &wave, &cpf);
+  return cpf;
+}
+
 template <int OP, int PHASE>
 static int gn_launch(bool cooperative, int grid, size_t smem, cudaStream_t st, const float* x, const float* gamma, const float* beta,
                      void* y, void* raw, float* partial, unsigned int* arrive, int P, int C, int F, int wave, int cpf, float eps,

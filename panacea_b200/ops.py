@@ -13,7 +13,7 @@ from . import _lib
 
 BF16 = torch.bfloat16
 F32 = torch.float32
-OP_BF16, OP_SPLIT3, OP_F32 = 0, 1, 2      # include/panacea_b200.h pn_operand_mode
+OP_BF16, OP_SPLIT3, OP_F32, OP_SPLIT3_B = 0, 1, 2, 3      # include/panacea_b200.h pn_operand_mode
 # include/panacea_b200.h pn_sampler_mode
 SAMPLER_EULER, SAMPLER_HEUN, SAMPLER_LMS, SAMPLER_DPM, SAMPLER_DPM_2M, SAMPLER_SCALE = range(6)
 
@@ -203,6 +203,10 @@ class NativeOps:
         self.launches += 2        # counter memset + kernel
         return (y, raw) if want_raw else y
 
+    def groupnorm_ctas_per_frame(self, frames, pixels, channels):
+        """pixel ranges each frame's GroupNorm statistics are split into for a [frames, pixels, channels] call"""
+        return int(self.lib.pn_groupnorm_ctas_per_frame(frames, pixels, channels))
+
     def groupnorm_pixel(self, x, gamma, beta, eps, silu):
         """x fp32 [b, T, P, C] -> bf16; statistics over (C/32, T) per pixel (temporal branch of ResBlock3D)."""
         _req(x.is_cuda and x.dtype == F32 and x.is_contiguous() and x.dim() == 4, "groupnorm_pixel: x fp32 [b,T,P,C]")
@@ -374,12 +378,15 @@ class NativeOps:
         self.launches += 1
         return x
 
-    def cast_operand(self, x):
-        """fp32 [..., C] -> GEMM operand (bf16 [..., C]; [..., 3C] in parity mode)."""
+    def cast_operand(self, x, weight_form=False):
+        """fp32 [..., C] -> GEMM operand (bf16 [..., C]; [..., 3C] in parity mode). weight_form: the B-operand layout
+        [hi | hi | lo] that split3() gives weights, for a GEMM whose B factor is an activation (bf16 mode: the same
+        bf16 tensor either way)."""
         _req(x.dtype == F32 and x.is_contiguous(), "cast_operand: fp32 contiguous")
         Cc = x.shape[-1]
+        mode = OP_SPLIT3_B if weight_form and self.operand_mode == OP_SPLIT3 else self.operand_mode
         y = self._operand_empty(x.shape, x.device)
-        _lib.check(self.lib.pn_cast_operand(_ptr(x), _ptr(y), x.numel() // Cc, Cc, self.operand_mode, _stream()), "pn_cast_operand")
+        _lib.check(self.lib.pn_cast_operand(_ptr(x), _ptr(y), x.numel() // Cc, Cc, mode, _stream()), "pn_cast_operand")
         self.launches += 1
         return y
 
@@ -531,6 +538,15 @@ class ParityOps(NativeOps):
             return y
         _req(out_dtype == F32, "parity gemm: outputs are fp32 (operands are produced by cast_operand)")
         return super().gemm(a, w, out_dtype=F32, **kw)
+
+    def softmax_rows(self, s, scale):
+        """fp32 [rows, N] -> split3 operand bf16 [rows, 3N] = [hi | lo | hi] of softmax(scale * s) per row."""
+        _req(s.is_cuda and s.dtype == F32 and s.dim() == 2 and s.is_contiguous() and s.shape[1] % 4 == 0, "softmax_rows: fp32 [rows, N]")
+        out = self._operand_empty(s.shape, s.device)
+        _lib.check(self.lib.pn_softmax_rows_operand(_ptr(s), _ptr(out), s.shape[0], s.shape[1], s.stride(0), out.stride(0), float(scale),
+                                                   self.operand_mode, _stream()), "pn_softmax_rows_operand")
+        self.launches += 1
+        return out
 
     # ------------------------------------------------------------------ attention (fp32, CUDA cores)
     def _attention_f32(self, q, k, v, out, *, q_ld, kv_ld, F, H, V, W, Hk, Vk, Wk, heads, head_dim, views):

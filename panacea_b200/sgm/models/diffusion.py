@@ -46,6 +46,8 @@ class DiffusionEngine3D(nn.Module):
         self.first_stage_model = instantiate_from_config(first_stage_config).eval()      # diffusion.py:124-130
         for p in self.first_stage_model.parameters():
             p.requires_grad = False
+        if precision is not None:
+            self.first_stage_model.set_precision(precision)                       # VAEEmbedder shares this model
         self.scale_factor = scale_factor
         self.disable_first_stage_autocast = disable_first_stage_autocast
         for emb in self.conditioner.embedders:                                     # diffusion.py:111-122 setup_vaeembedder

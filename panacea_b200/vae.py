@@ -9,8 +9,10 @@ AttnBlock / ResnetBlock, then per level 3 ResnetBlocks (+ nearest-2x Upsample + 
 `pn_conv3x3_direct` for the 4-channel input and 3-channel output convs, and — for the single-head attention of the mid
 block whose head_dim is the full channel count (512) — two GEMMs around `pn_softmax_rows` per frame:
 S = q k^T, P = softmax(S / sqrt(C)), O = P v (the value bias is added after the product: rows of P sum to one).
-bf16 operands, fp32 accumulation and residual stream, like the UNet's fast path. Parameters are addressed by the
-reference's state-dict names (`decoder.*`, `post_quant_conv.*`), so SD-VAE checkpoints load unchanged."""
+The op set decides the precision, as on the UNet: NativeOps gives bf16 operands with fp32 accumulation and residual
+stream; ParityOps gives split-bf16 operands (fp32-class products), the reference's fp32 VAE to rtol 1e-3 / atol 1e-4.
+Parameters are addressed by the reference's state-dict names (`decoder.*`, `post_quant_conv.*`), so SD-VAE checkpoints
+load unchanged."""
 from __future__ import annotations
 
 import torch
@@ -125,6 +127,26 @@ class _VAEBlocks:
         w3[:, :, 1, 1] = w[:, :, 0, 0]
         return _pack_direct(w3)
 
+    def frame_chunks(self, frames: int, hw: tuple, max_frames: int) -> list:
+        """Split `frames` into calls of at most `max_frames` frames that give bitwise the output of one call over all
+        of them, or [frames] if there is no such split. Every op of the network is per frame: pn_gemm has no split-K
+        and sums each row in the same order whatever the row count, the convs pad at frame edges, the attention loops
+        over frames. The one exception is GroupNorm: pn_groupnorm_silu reduces each frame over `cpf` pixel ranges, and
+        `cpf` depends on how many frames the call holds. A chunk size is allowed when it gives the same `cpf` as all
+        frames for every (pixels, channels) the network normalises."""
+        if frames <= max_frames:
+            return [frames]
+        shapes = self._gn_shapes(hw)
+        cpf = self.ops.groupnorm_ctas_per_frame
+        want = [cpf(frames, P, C) for P, C in shapes]
+        ok = [c for c in range(max_frames, 0, -1) if all(cpf(c, P, C) == w for (P, C), w in zip(shapes, want))]
+        best = {0: []}                                  # fewest calls that add up to n frames, allowed sizes only
+        for n in range(1, frames + 1):
+            cands = [best[n - c] + [c] for c in ok if c <= n and n - c in best]
+            if cands:
+                best[n] = min(cands, key=len)
+        return best.get(frames, [frames])
+
 
 class VAEDecoderEngine(_VAEBlocks):
     def __init__(self, ddconfig: dict, ops, embed_dim: int = 4):
@@ -161,6 +183,8 @@ class VAEDecoderEngine(_VAEBlocks):
         P = H * Wd
         if P % 64 or C % 64:
             raise NotImplementedError("VAE mid attention needs H*W and C to be multiples of 64")
+        if ops.operand_mult == 3:
+            return self._attn_split3(k, x)
         a = ops.groupnorm(x, W[k + ".norm.g"], W[k + ".norm.b"], 1e-6, False).view(Fr, P, C)
         out = torch.empty_like(x)
         dt = a.dtype
@@ -174,6 +198,42 @@ class VAEDecoderEngine(_VAEBlocks):
             o = ops.gemm(p, vT, bias=W[k + ".v.b"], out_dtype=dt)              # rows of p sum to 1: + b_v after the product
             ops.gemm(o, W[k + ".proj_out.w"], bias=W[k + ".proj_out.b"], residual=x[f].reshape(P, C), out=out[f].view(P, C))
         return out
+
+    def _attn_split3(self, k, x):
+        """AttnBlock.forward in parity mode (split-bf16 operands, fp32-class products). Both factors of S = q k^T and of
+        O = P v are activations, so one of each pair is cast to the weight form [hi | hi | lo] on the device; the
+        other is in the A form [hi | lo | hi] that every producer writes."""
+        ops, W = self.ops, self.W
+        Fr, H, Wd, C = x.shape
+        P = H * Wd
+        a = ops.groupnorm(x, W[k + ".norm.g"], W[k + ".norm.b"], 1e-6, False).view(Fr, P, -1)
+        out = torch.empty_like(x)
+        for f in range(Fr):
+            af = a[f]
+            q = ops.gemm(af, W[k + ".q.w"], bias=W[k + ".q.b"])                  # fp32 [P, C]
+            kk = ops.gemm(af, W[k + ".k.w"], bias=W[k + ".k.b"])
+            v = ops.gemm(af, W[k + ".v.w"])                                     # value bias added after the product
+            s = ops.gemm(ops.cast_operand(q), ops.cast_operand(kk, weight_form=True))      # [P, P] fp32 scores
+            del q, kk
+            p = ops.softmax_rows(s, C ** -0.5)                                  # split3 [P, 3P]
+            del s
+            vT = ops.nhwc_to_nchw(v.view(1, 1, P, C)).view(C, P)                # [C, P]
+            o = ops.gemm(p, ops.cast_operand(vT, weight_form=True), bias=W[k + ".v.b"])     # rows of p sum to 1
+            del p
+            ops.gemm(ops.cast_operand(o), W[k + ".proj_out.w"], bias=W[k + ".proj_out.b"], residual=x[f].reshape(P, C),
+                     out=out[f].view(P, C))
+        return out
+
+    def _gn_shapes(self, hw):
+        """(pixels per frame, channels) of every GroupNorm of a decode from a latent of `hw` (decode() below)"""
+        (h, w), ch, ch_mult, nrb = hw, self.dd["ch"], tuple(self.dd["ch_mult"]), self.dd["num_res_blocks"]
+        block_in = ch * ch_mult[-1]
+        shapes = {(h * w, block_in)}                                         # mid block
+        for i, lvl in enumerate(reversed(range(len(ch_mult)))):
+            P, block_out = (h << i) * (w << i), ch * ch_mult[lvl]
+            shapes |= {(P, block_in), (P, block_out)}                        # norm1 of the first block, every other norm
+            block_in = block_out
+        return sorted(shapes)                                                # norm_out: (last P, ch * ch_mult[0]) is in it
 
     # ------------------------------------------------------------------------------------------ network
     @torch.no_grad()
@@ -205,6 +265,7 @@ class VAEEncoderEngine(_VAEBlocks):
     conv_out -> the posterior's moments [F, 2 z_channels, h/8, w/8]; sampling the posterior is the caller's one-liner."""
     _res = VAEDecoderEngine._res
     _attn = VAEDecoderEngine._attn
+    _attn_split3 = VAEDecoderEngine._attn_split3
 
     def __init__(self, ddconfig: dict, ops, embed_dim: int = 4):
         self.dd, self.ops, self.embed_dim = dict(ddconfig), ops, embed_dim
@@ -218,6 +279,19 @@ class VAEEncoderEngine(_VAEBlocks):
         W["in.w"], W["in.b"] = _pack_direct(P["encoder.conv_in.weight"].detach(), cin_pad=(cin + 3) // 4 * 4), f(P["encoder.conv_in.bias"])
         W["q.w"], W["q.b"] = self._pack_1x1_direct(P["quant_conv.weight"]), f(P["quant_conv.bias"])
         self.W = W
+
+    def _gn_shapes(self, hw):
+        """(pixels per frame, channels) of every GroupNorm of an encode of an image of `hw` (encode_moments() below;
+        Downsample: (n - 2) // 2 + 1)"""
+        (h, w), ch, ch_mult = hw, self.dd["ch"], tuple(self.dd["ch_mult"])
+        shapes, block_in = set(), ch
+        for lvl in range(len(ch_mult)):
+            block_out = ch * ch_mult[lvl]
+            shapes |= {(h * w, block_in), (h * w, block_out)}                # norm1 of the first block, every other norm
+            block_in = block_out
+            if lvl != len(ch_mult) - 1:
+                h, w = (h - 2) // 2 + 1, (w - 2) // 2 + 1
+        return sorted(shapes)                                                # mid block and norm_out: (last P, block_in)
 
     @torch.no_grad()
     def encode_moments(self, x_nchw: torch.Tensor) -> torch.Tensor:

@@ -79,7 +79,9 @@ typedef struct pn_gemm_args {
   int32_t residual_bf16;  /* the residual is bf16 (bf16 output only): the transformer blocks' bf16 token stream */
   /* LayerNorm folded into the GEMMs around the bf16 token stream (attention.py:699-701 + :726-747, norm1/2/3):
    * ln_stats_out — this GEMM (bf16 out, no GEGLU) also writes, per output row, pn_gemm_ln_parts(N) partial
-   *   (sum, sum of squares) pairs of the bf16 values it stores: float [rows][parts][2];
+   *   (sum, sum of squares) pairs: float [rows][parts][2]. With BN = 160 if N % 160 == 0 else 128, part 2 * t + h
+   *   sums columns [t * BN + h * BN/2, t * BN + (h + 1) * BN/2) (half h of column tile t), taken from the fp32 values
+   *   before their bf16 rounding (only the per-row totals are meaningful to a consumer);
    * ln_stats_in / ln_parts_in / ln_colsum / ln_eps — (1x1, bf16 out, no GEGLU) A is the UN-normalised stream, B = W diag(gamma); the epilogue
    *   finishes the LayerNorm: out = rstd_m (acc - mean_m s_n) + bias_n with s_n = ln_colsum[n] = sum_k B[n,k] and the
    *   caller's bias_n = sum_k beta_k W[n,k] (+ the layer's own bias); mean/rstd over the C = K channels of row m. */

@@ -13,23 +13,23 @@ F32 = torch.float32
 
 class TextRefOps(TorchRefOps):
     def layernorm(self, x, gamma, beta, eps=1e-5, out_f32=False):
-        return F.layer_norm(x.float(), (x.shape[-1],), gamma, beta, eps)
+        return F.layer_norm(self._c(x), (x.shape[-1],), self._c(gamma), self._c(beta), eps)
 
     def attention_causal(self, qkv, heads):
         b, L, C3 = qkv.shape
         C = C3 // 3
-        q, k, v = (t.reshape(b, L, heads, C // heads).transpose(1, 2) for t in qkv.float().split(C, dim=-1))
+        q, k, v = (t.reshape(b, L, heads, C // heads).transpose(1, 2) for t in self._c(qkv).split(C, dim=-1))
         o = F.scaled_dot_product_attention(q, k, v, is_causal=True)
         return o.transpose(1, 2).reshape(b, L, C)
 
     def gelu_operand(self, x):
-        return F.gelu(x.float())
+        return F.gelu(self._c(x))
 
     def token_embedding(self, tokens, table, pos):
         vocab = table.shape[0]
         if int(tokens.min()) < 0 or int(tokens.max()) >= vocab:
             raise ValueError(f"token_embedding: token ids must lie in [0, {vocab})")
-        return table[tokens] + pos[:tokens.shape[1]]
+        return self._c(table)[tokens] + self._c(pos)[:tokens.shape[1]]
 
 
 class TextSplitOps(TorchSplitOps, TextRefOps):

@@ -65,8 +65,8 @@ def test_gemm_bf16_out_and_rowvec(ops):
 
 @pytest.mark.parametrize("M,N,K", [(3000, 320, 320), (2048, 640, 640), (1500, 1280, 1280), (172032 // 4, 320, 1280), (130, 320, 320)])
 def test_gemm_bf16_token_stream_residual(ops, M, N, K):
-    """bf16 output with a bf16 residual updated in place (the transformer blocks' token stream): streaming epilogue
-    (K <= 640 and larger K)."""
+    """bf16 output with a bf16 residual updated in place (the transformer blocks' token stream), in place and not,
+    for K <= 640 and larger K."""
     a = _rand((M, K), 13); w = _rand((N, K), 14, K ** -0.5)
     bias = _rand((N,), 15, dtype=torch.float32)
     y = _rand((M, N), 16)
@@ -83,9 +83,8 @@ def test_gemm_bf16_token_stream_residual(ops, M, N, K):
 
 @pytest.mark.parametrize("M,C", [(3000, 320), (2500, 640), (172032 // 8, 320), (700, 128), (130, 512)])
 def test_gemm_layernorm_fold(ops, M, C):
-    """LayerNorm folded into the GEMMs around the bf16 token stream: (i) a producer (bf16 out + bf16 residual, streaming
-    epilogue) emits per-row partial sums of what it stores; (ii) a consumer (bf16 streaming epilogue) takes the
-    un-normalised stream, W diag(gamma), the column sums and W beta, and must equal Linear(LayerNorm(stream))."""
+    """LayerNorm folded into the GEMMs around the bf16 token stream: (i) a producer (bf16 out + bf16 residual) emits
+    per-row partial sums of the values it rounds and stores; (ii) a consumer (bf16 out) takes the un-normalised stream, W diag(gamma), the column sums and W beta, and must equal Linear(LayerNorm(stream))."""
     from panacea_b200.engine import Engine
     a = _rand((M, C), 30); wo = _rand((C, C), 31, C ** -0.5)
     y0 = _rand((M, C), 32, 2.0) + 0.7
@@ -122,9 +121,8 @@ def test_gemm_geglu(ops):
 
 @pytest.mark.parametrize("kind", ["fp32_res", "bf16", "geglu", "fp32_wide"])
 def test_gemm_weight_stationary_schedule(ops, kind):
-    """K = 320 with many row tiles takes the weight-stationary schedule (contiguous column-major tile ranges, the
-    weight tile resident in shared memory); M is not a multiple of the 256-row pair tile and the last unit's range
-    crosses a column-tile boundary."""
+    """K = 320 over many waves of row tiles (8 x 148 x 128 + 333 rows): the last 128-row tile is partial, and each
+    epilogue (fp32 + residual, bf16, GEGLU) spans several 160-wide column tiles (N = 480, 960, 2560)."""
     M, K = 8 * 148 * 128 + 333, 320
     a = _rand((M, K), 40)
     if kind == "geglu":
@@ -175,7 +173,8 @@ def test_gemm_strided_view(ops):
 
 @pytest.mark.parametrize("NB,H,W,C,N", [(2, 8, 24, 64, 160), (3, 4, 42, 128, 320), (2, 32, 336, 320, 320),
                                         (4, 16, 168, 64, 64), (16, 4, 42, 64, 160),
-                                        # H % 16 == 0, W % 8 == 0, N % 160 == 0: the haloed-tile conv path (MODE 6)
+                                        # narrow images: the 128-row tile is a box of several image rows, so the taps
+                                        # read across its top, bottom and side edges
                                         (1, 16, 24, 64, 160), (2, 32, 40, 128, 320), (1, 48, 16, 64, 640), (3, 16, 168, 192, 640)])
 def test_conv3x3(ops, NB, H, W, C, N):
     x = _rand((NB, H, W, C), 15)
@@ -203,7 +202,7 @@ def test_temporal_conv(ops, b, T, P, C):
 
 @pytest.mark.parametrize("M,N,K,G", [(2048, 320, 320, 8), (1536, 640, 64, 3), (640, 128, 128, 5)])
 def test_gemm_fp32_rowvec_residual_streaming_epilogue(ops, M, N, K, G):
-    """fp32 output + per-row-group vector (time-emb / pos-emb) + in-place residual: the TMA streaming epilogue."""
+    """fp32 output + per-row-group vector (time-emb / pos-emb, strided rows) + in-place residual."""
     a = _rand((M, K), 30); w = _rand((N, K), 31, K ** -0.5)
     bias = _rand((N,), 32, dtype=torch.float32)
     rv_full = _rand((G, N + 64), 33, dtype=torch.float32)

@@ -16,7 +16,11 @@ F32 = torch.float32
 
 
 class TorchRefOps:
-    """fp32 everywhere: operands are plain fp32 tensors, weights stay fp32."""
+    """fp32 everywhere: operands are plain fp32 tensors, weights stay fp32. Results are allocated on the inputs' device
+    and computed in `dtype`; with `pre_store` a method returns its value in `dtype` before the rounding to the output
+    dtype the kernel stores (TorchRefOps64, the fp64 reference of the per-call replay check, tests/op_check.py)."""
+    dtype = F32
+    pre_store = False
     operand_mult = 1
     qkv_dtype = F32
     act_dtype = F32
@@ -26,6 +30,12 @@ class TorchRefOps:
 
     def __init__(self):
         self.launches = 0
+
+    def _c(self, t):
+        return None if t is None else t.to(self.dtype)
+
+    def _store(self, y, dtype):
+        return y if self.pre_store else y.to(dtype)
 
     def pack_matrix(self, w, taps=1):
         return w.detach().to(F32).contiguous()
@@ -38,12 +48,13 @@ class TorchRefOps:
         th, tw = taps
         C = a.shape[-1]
         N = w.shape[0]
-        wf = w.float()
+        wf = self._c(w)
         if (th, tw) == (1, 1):
             lead = a.shape[:-1]
-            y = a.float().reshape(-1, C) @ wf.t()
+            y = self._c(a).reshape(-1, C) @ wf.t()
             if ln is not None:      # pn_gemm_args.ln_*: finish the folded LayerNorm from the producer's partial row sums
                 st, colsum, eps = ln
+                st, colsum = self._c(st), self._c(colsum)
                 sm, sq = st[..., 0].sum(1), st[..., 1].sum(1)
                 mu = sm / C
                 rstd = torch.rsqrt((sq / C - mu * mu).clamp_min(0) + eps)
@@ -51,37 +62,37 @@ class TorchRefOps:
         else:
             NB, H, W, _ = a.shape
             lead = (NB, H, W)
-            ap = F.pad(a.float(), (0, 0, tw // 2, tw // 2, th // 2, th // 2))
-            y = torch.zeros(NB * H * W, N)
+            ap = F.pad(self._c(a), (0, 0, tw // 2, tw // 2, th // 2, th // 2))
+            y = torch.zeros(NB * H * W, N, device=a.device, dtype=self.dtype)
             for i in range(th):
                 for j in range(tw):
                     tap = i * tw + j
                     y += ap[:, i:i + H, j:j + W, :].reshape(-1, C) @ wf[:, tap * C:(tap + 1) * C].t()
         rows = y.shape[0]
         if bias is not None:
-            y = y + bias
+            y = y + self._c(bias)
         if rowvec is not None:
-            grp = (torch.arange(rows) // rows_per_group) % n_groups
-            y = y + rowvec[grp]
+            grp = (torch.arange(rows, device=y.device) // rows_per_group) % n_groups
+            y = y + self._c(rowvec)[grp]
         if geglu:
             y3 = y.reshape(rows, -1, 2, 16)          # packed layout: 16 value columns, then their 16 gate columns
             y = (y3[:, :, 0] * F.gelu(y3[:, :, 1])).reshape(rows, -1)
         if residual is not None:
-            y = y + residual.reshape(rows, -1)
+            y = y + self._c(residual).reshape(rows, -1)
         if residual2 is not None:
-            y = y + residual2.reshape(rows, -1)
-        y = y.to(out_dtype)
+            y = y + self._c(residual2).reshape(rows, -1)
         stats = None
-        if ln_stats_out:            # two partial (sum, sumsq) pairs per 160-wide column tile, like the streaming epilogue
-            yy = y.float()
-            n = yy.shape[1]
+        if ln_stats_out:
+            # include/panacea_b200.h pn_gemm_args.ln_stats_out: part 2 * tile + h holds (sum, sum of squares) of the values
+            # before the store rounding over columns [h * BN/2, (h + 1) * BN/2) of column tile `tile`, BN = 160 or 128
+            n = y.shape[1]
             bn = 160 if n % 160 == 0 else 128
             parts = []
-            for c0 in range(0, n, bn):
-                for chunks in ((0, 2, 4), (1, 3)) if bn == 160 else ((0, 2), (1, 3)):
-                    cols = torch.cat([yy[:, c0 + 32 * c:c0 + 32 * c + 32] for c in chunks], 1)
-                    parts.append(torch.stack([cols.sum(1), (cols * cols).sum(1)], -1))
+            for c0 in range(0, n, bn // 2):
+                cols = y[:, c0:c0 + bn // 2]
+                parts.append(torch.stack([cols.sum(1), (cols * cols).sum(1)], -1))
             stats = torch.stack(parts, 1).contiguous()
+        y = self._store(y, out_dtype)
         if out is not None:
             out.reshape(rows, -1).copy_(y)
             res = out.reshape(*lead, y.shape[1])
@@ -91,8 +102,9 @@ class TorchRefOps:
 
     def groupnorm(self, x, gamma, beta, eps, silu, want_raw=False, out_f32=False):
         Fr, C = x.shape[0], x.shape[-1]
+        x = self._c(x)
         z = x.reshape(Fr, -1, C).permute(0, 2, 1)
-        y = F.group_norm(z, 32, gamma, beta, eps)
+        y = F.group_norm(z, 32, self._c(gamma), self._c(beta), eps)
         if silu:
             y = F.silu(y)
         y = y.permute(0, 2, 1).reshape(x.shape).contiguous()
@@ -100,14 +112,14 @@ class TorchRefOps:
 
     def groupnorm_pixel(self, x, gamma, beta, eps, silu):
         b, T, P, C = x.shape
-        z = x.permute(0, 2, 3, 1).reshape(b * P, C, T)
-        y = F.group_norm(z, 32, gamma, beta, eps)
+        z = self._c(x).permute(0, 2, 3, 1).reshape(b * P, C, T)
+        y = F.group_norm(z, 32, self._c(gamma), self._c(beta), eps)
         if silu:
             y = F.silu(y)
         return y.reshape(b, P, C, T).permute(0, 3, 1, 2).contiguous()
 
     def layernorm(self, x, gamma, beta, eps=1e-5):
-        return F.layer_norm(x, (x.shape[-1],), gamma, beta, eps)
+        return F.layer_norm(self._c(x), (x.shape[-1],), self._c(gamma), self._c(beta), eps)
 
     @staticmethod
     def _mha(q, k, v, heads):
@@ -122,37 +134,37 @@ class TorchRefOps:
     def attention_view(self, qkv, heads, cross, neighbours):
         Fr, H, V, w, C3 = qkv.shape
         C = C3 // 3
-        q, k, v = qkv.float().split(C, dim=-1)
-        out = torch.empty(Fr, H, V, w, C)
+        q, k, v = self._c(qkv).split(C, dim=-1)
+        out = torch.empty(Fr, H, V, w, C, device=qkv.device, dtype=self.dtype)
         for i in range(V):
             nb = neighbours[i] if cross else (i,)
             ki = torch.cat([k[:, :, j] for j in nb], dim=2).reshape(Fr, -1, C)
             vi = torch.cat([v[:, :, j] for j in nb], dim=2).reshape(Fr, -1, C)
             out[:, :, i] = self._mha(q[:, :, i].reshape(Fr, H * w, C), ki, vi, heads).reshape(Fr, H, w, C)
-        return out.to(qkv.dtype)
+        return self._store(out, qkv.dtype)
 
     def attention_text(self, q, kv, heads):
         C = q.shape[-1]
-        return self._mha(q.float(), kv.float()[..., :C], kv.float()[..., C:], heads).to(q.dtype)
+        return self._store(self._mha(self._c(q), self._c(kv)[..., :C], self._c(kv)[..., C:], heads), q.dtype)
 
     def attention_temporal(self, qkv, heads):
         b, T, P, C3 = qkv.shape
         C = C3 // 3
-        q, k, v = qkv.float().split(C, dim=-1)
+        q, k, v = self._c(qkv).split(C, dim=-1)
         seq = lambda z: z.permute(0, 2, 1, 3).reshape(b * P, T, C)
         o = self._mha(seq(q), seq(k), seq(v), heads)
-        return o.reshape(b, P, T, C).permute(0, 2, 1, 3).contiguous().to(qkv.dtype)
+        return self._store(o.reshape(b, P, T, C).permute(0, 2, 1, 3).contiguous(), qkv.dtype)
 
     def conv3x3_direct(self, x, w_packed, bias, cout, *, stride=1, silu=False, addend=None, out_dtype=F32):
         cin = x.shape[-1]
-        w = w_packed[:, :cin, :cout].reshape(3, 3, cin, cout).permute(3, 2, 0, 1)
-        y = F.conv2d(x.float().permute(0, 3, 1, 2), w, bias, stride=stride, padding=1)
+        w = self._c(w_packed)[:, :cin, :cout].reshape(3, 3, cin, cout).permute(3, 2, 0, 1)
+        y = F.conv2d(self._c(x).permute(0, 3, 1, 2), w, self._c(bias), stride=stride, padding=1)
         if silu:
             y = F.silu(y)
         y = y.permute(0, 2, 3, 1)
         if addend is not None:
-            y = y + addend
-        return y.contiguous().to(out_dtype)
+            y = y + self._c(addend)
+        return self._store(y.contiguous(), out_dtype)
 
     def im2col_s2(self, x, pad=1):
         Fr, H, W, C = x.shape
@@ -178,7 +190,7 @@ class TorchRefOps:
         return x
 
     def softmax_rows(self, s, scale):
-        return torch.softmax(s.float() * scale, dim=-1)
+        return torch.softmax(self._c(s) * scale, dim=-1)
 
     def nchw_to_nhwc(self, x, out=None, ch_off=0):
         y = x.permute(0, 2, 3, 1)
@@ -192,12 +204,13 @@ class TorchRefOps:
 
     def timestep_embedding(self, t, dim):
         half = dim // 2
-        freqs = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=F32) / half)
-        args = t[:, None].float() * freqs[None]
+        freqs = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=F32) / half).to(t.device)
+        args = self._c(t[:, None].float() * freqs[None])       # the fp32 product, as the kernel forms it
         return torch.cat([torch.cos(args), torch.sin(args)], dim=-1)
 
     def linear_small(self, x, w, bias, silu_in=False, silu_out=False):
-        y = F.linear(F.silu(x) if silu_in else x, w.float(), bias)
+        x = self._c(x)
+        y = F.linear(F.silu(x) if silu_in else x, self._c(w), self._c(bias))
         return F.silu(y) if silu_out else y
 
     def cfg_euler_step(self, x, net2, x_in_next, sigma, sigma_next, scale, c_in_next, sigma_q=None, net_is_denoised=False):
@@ -213,6 +226,13 @@ class TorchRefOps:
 
     def scale_dup(self, x, s, copies):
         return torch.cat([x * s] * copies)
+
+
+class TorchRefOps64(TorchRefOps):
+    """The same semantics in fp64, results before the store rounding: the reference each kernel call is checked against.
+    Convolutions stay one matmul per tap, so on a GPU they run as fp64 GEMMs."""
+    dtype = torch.float64
+    pre_store = True
 
 
 class TorchFoldOps(TorchRefOps):

@@ -124,9 +124,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
 
   // ===================== consumer warpgroups =====================
   const int wg = warp >> 2;
+  // Not zero-filled: a tile's first wgmma runs with scale-d = 0 and overwrites it. A fill here would be a non-wgmma
+  // definition of the accumulator registers, which makes ptxas serialise every wgmma of the loop (C7515).
   float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   {
     const uint32_t base = smem_u32(smem);
     const uint64_t descA0 = wgmma_desc(base + wg * (64 * 128), 16, 1024, kSw128);

@@ -32,7 +32,6 @@ struct AfParams {
 
 template <int D, int OP>
 __global__ void __launch_bounds__(AF_QTILE) attn_f32_view_kernel(const AfParams p) {
-  pdl_prologue_done();
   __shared__ __align__(16) float sK[AF_KTILE][D];
   __shared__ __align__(16) float sV[AF_KTILE][D];
   const int tiles = (p.H * p.W + AF_QTILE - 1) / AF_QTILE;
@@ -124,7 +123,6 @@ template <int D, int OP>
 __global__ void __launch_bounds__(128) attn_f32_temporal_kernel(const float* __restrict__ q, const float* __restrict__ k,
                                                                 const float* __restrict__ v, void* __restrict__ out, int batch,
                                                                 int T, int P, int heads, long long ld, float scale_log2) {
-  pdl_prologue_done();
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long total = (long long)batch * T * P * heads;
   if (idx >= total) return;
@@ -185,7 +183,6 @@ __global__ void __launch_bounds__(128) attn_f32_causal_kernel(const float* __res
                                                               const float* __restrict__ v, void* __restrict__ out, int batch,
                                                               int L, int heads, long long ld, float scale_log2) {
   constexpr int D = 64;
-  pdl_prologue_done();
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long total = (long long)batch * heads * L;
   if (idx >= total) return;
@@ -251,8 +248,8 @@ extern "C" int pn_attention_causal_f32(const float* q, const float* k, const flo
   const long long blocks = (total + 127) / 128;
   PN_REQUIRE(blocks < (1ll << 31), "pn_attention_causal_f32: grid too large");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  PN_DISPATCH_OP(operand_mode, (launch_kernel(attn_f32_causal_kernel<OP>, dim3((unsigned)blocks), dim3(128), 0, st, 1, q, k, v, out,
-                                              (int)batch, (int)L, heads, ld, scale * 1.4426950408889634f)));
+  PN_DISPATCH_OP(operand_mode, attn_f32_causal_kernel<OP><<<(unsigned)blocks, 128, 0, st>>>(q, k, v, out, (int)batch, (int)L, heads, ld,
+                                                                                         scale * 1.4426950408889634f));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
@@ -288,8 +285,8 @@ extern "C" int pn_attention_f32(const pn_attn_args* a, int operand_mode, void* s
   const long long blocks = tiles * a->heads * a->V * a->F;
   PN_REQUIRE(blocks > 0 && blocks < (1ll << 31), "pn_attention_f32: grid too large");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  if (a->head_dim == 64) PN_DISPATCH_OP(operand_mode, (launch_kernel(attn_f32_view_kernel<64, OP>, dim3((unsigned)blocks), dim3(AF_QTILE), 0, st, 1, p)));
-  else PN_DISPATCH_OP(operand_mode, (launch_kernel(attn_f32_view_kernel<80, OP>, dim3((unsigned)blocks), dim3(AF_QTILE), 0, st, 1, p)));
+  if (a->head_dim == 64) PN_DISPATCH_OP(operand_mode, attn_f32_view_kernel<64, OP><<<(unsigned)blocks, AF_QTILE, 0, st>>>(p));
+  else PN_DISPATCH_OP(operand_mode, attn_f32_view_kernel<80, OP><<<(unsigned)blocks, AF_QTILE, 0, st>>>(p));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
@@ -308,9 +305,9 @@ extern "C" int pn_attention_temporal_f32(const float* q, const float* k, const f
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   const float sl2 = scale * 1.4426950408889634f;
   if (head_dim == 64)
-    PN_DISPATCH_OP(operand_mode, (launch_kernel(attn_f32_temporal_kernel<64, OP>, dim3((unsigned)blocks), dim3(128), 0, st, 1, q, k, v, out, (int)batch, (int)T, (int)pixels, heads, ld, sl2)));
+    PN_DISPATCH_OP(operand_mode, attn_f32_temporal_kernel<64, OP><<<(unsigned)blocks, 128, 0, st>>>(q, k, v, out, (int)batch, (int)T, (int)pixels, heads, ld, sl2));
   else
-    PN_DISPATCH_OP(operand_mode, (launch_kernel(attn_f32_temporal_kernel<80, OP>, dim3((unsigned)blocks), dim3(128), 0, st, 1, q, k, v, out, (int)batch, (int)T, (int)pixels, heads, ld, sl2)));
+    PN_DISPATCH_OP(operand_mode, attn_f32_temporal_kernel<80, OP><<<(unsigned)blocks, 128, 0, st>>>(q, k, v, out, (int)batch, (int)T, (int)pixels, heads, ld, sl2));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }

@@ -88,7 +88,6 @@ __global__ void __launch_bounds__(FA_THREADS, 1) attn_fa_kernel(const __grid_con
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_prologue_done();
 
   // query tile fastest, then head, view, frame: CTAs that run concurrently share K/V in L2
   int item = blockIdx.x;
@@ -338,6 +337,7 @@ extern "C" int pn_attention(const pn_attn_args* a, void* stream_v) {
     const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem_total);
     if (rc != PN_OK) return rc;
   }
-  PN_CHECK_CUDA(launch_kernel(kern, dim3((unsigned)items), dim3(FA_THREADS), smem_total, reinterpret_cast<cudaStream_t>(stream_v), 1, p));
+  kern<<<(unsigned)items, FA_THREADS, smem_total, reinterpret_cast<cudaStream_t>(stream_v)>>>(p);
+  PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }

@@ -41,7 +41,6 @@ __global__ void __launch_bounds__(TA_WARPS * 32) attn_temporal_kernel(const __nv
                                                                       const __nv_bfloat16* __restrict__ v,
                                                                       __nv_bfloat16* __restrict__ out, int nb, int T, int P,
                                                                       int heads, long long ld, long long out_ld, float scale) {
-  pdl_prologue_done();
   constexpr int TA_PITCH = D + 8;
   constexpr int RCH = D / 8;            // 16-byte chunks per row
   __shared__ __align__(16) __nv_bfloat16 sq[TA_WARPS][TA_MAXT][TA_PITCH];   // Q rows, later the output rows
@@ -155,7 +154,6 @@ __global__ void __launch_bounds__((CA_MAXL / 16) * 32) attn_causal_kernel(const 
                                                                           const __nv_bfloat16* __restrict__ v,
                                                                           __nv_bfloat16* __restrict__ out, int L, int heads,
                                                                           long long ld, long long out_ld, float scale) {
-  pdl_prologue_done();
   constexpr int RCH = CA_D / 8;
   extern __shared__ __align__(16) unsigned char ca_smem[];
   const int Lp = (L + 15) & ~15;
@@ -286,9 +284,9 @@ extern "C" int pn_attention_causal(const void* q, const void* k, const void* v, 
   const size_t smem = (size_t)3 * Lp * CA_PITCH * sizeof(__nv_bfloat16);
   const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(&attn_causal_kernel), smem);
   if (rc != PN_OK) return rc;
-  launch_kernel(attn_causal_kernel, dim3((unsigned)blocks), dim3((Lp / 16) * 32), smem, reinterpret_cast<cudaStream_t>(stream_v), 1,
-                reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
-                reinterpret_cast<const __nv_bfloat16*>(v), reinterpret_cast<__nv_bfloat16*>(out), (int)L, heads, ld, out_ld, scale);
+  attn_causal_kernel<<<(unsigned)blocks, (Lp / 16) * 32, smem, reinterpret_cast<cudaStream_t>(stream_v)>>>(
+      reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
+      reinterpret_cast<const __nv_bfloat16*>(v), reinterpret_cast<__nv_bfloat16*>(out), (int)L, heads, ld, out_ld, scale);
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
@@ -305,15 +303,15 @@ extern "C" int pn_attention_temporal(const void* q, const void* k, const void* v
   const long long blocks = (total + TA_WARPS - 1) / TA_WARPS;
   PN_REQUIRE(blocks < (1ll << 31), "pn_attention_temporal: grid too large");
   if (head_dim == 64)
-    launch_kernel(attn_temporal_kernel<64>, dim3((unsigned)blocks), dim3(TA_WARPS * 32), 0, reinterpret_cast<cudaStream_t>(stream_v), 1,
-                  reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
-                  reinterpret_cast<const __nv_bfloat16*>(v), reinterpret_cast<__nv_bfloat16*>(out), (int)batch, (int)T, (int)pixels, heads,
-                  ld, out_ld, scale);
+    attn_temporal_kernel<64><<<(unsigned)blocks, TA_WARPS * 32, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
+        reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
+        reinterpret_cast<const __nv_bfloat16*>(v), reinterpret_cast<__nv_bfloat16*>(out), (int)batch, (int)T, (int)pixels, heads,
+        ld, out_ld, scale);
   else
-    launch_kernel(attn_temporal_kernel<80>, dim3((unsigned)blocks), dim3(TA_WARPS * 32), 0, reinterpret_cast<cudaStream_t>(stream_v), 1,
-                  reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
-                  reinterpret_cast<const __nv_bfloat16*>(v), reinterpret_cast<__nv_bfloat16*>(out), (int)batch, (int)T, (int)pixels, heads,
-                  ld, out_ld, scale);
+    attn_temporal_kernel<80><<<(unsigned)blocks, TA_WARPS * 32, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
+        reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
+        reinterpret_cast<const __nv_bfloat16*>(v), reinterpret_cast<__nv_bfloat16*>(out), (int)batch, (int)T, (int)pixels, heads,
+        ld, out_ld, scale);
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }

@@ -2,7 +2,6 @@
 #include "../../include/panacea_b200.h"
 
 #include <cstdarg>
-#include <cstdlib>
 #include <mutex>
 #include <unordered_map>
 
@@ -176,10 +175,12 @@ int sm_count() {
   return g_sm_count[dev];
 }
 
-bool pdl_enabled() {
-  // opt-in (PN_PDL=1): the launches of the captured step graph are not launch-latency bound
-  static const bool on = [] { const char* e = std::getenv("PN_PDL"); return e && std::atoi(e) != 0; }();
-  return on;
+int stride_grid(size_t total, int threads) {
+  size_t g = (total + threads - 1) / threads;
+  const size_t cap = (size_t)16 * sm_count();
+  if (g > cap) g = cap;
+  if (g < 1) g = 1;
+  return (int)g;
 }
 
 int ensure_dyn_smem(const void* func, size_t bytes, bool max_carveout) {

@@ -41,39 +41,10 @@ int cached_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_
                      const uint64_t* strides_elems, const uint32_t* box, int swizzle_bytes);
 
 int sm_count();                                          // of the current device
+// blocks of `threads` for a grid-stride loop over `total` items: one item per thread, at most 16 blocks per SM
+int stride_grid(size_t total, int threads = 256);
 // opt in to `bytes` of dynamic shared memory for `func` on the current device (once per device and size);
 // `max_carveout` also asks for the largest shared-memory carveout, for kernels that plan on several CTAs per SM
 int ensure_dyn_smem(const void* func, size_t bytes, bool max_carveout = false);
-
-// PN_PDL=1 enables programmatic dependent launch (off by default: measured no gain on the captured graph)
-bool pdl_enabled();
-
-// Launch with programmatic stream serialization (and optionally a thread-block cluster): the kernel must call
-// pdl_prologue_done() (ptx.cuh) before its first global-memory access.
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, int cluster_x,
-                                 Args&&... args) {
-  cudaLaunchConfig_t cfg;
-  std::memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  int n = 0;
-  attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[n].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  ++n;
-  if (cluster_x > 1) {
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = (unsigned)cluster_x;
-    attr[n].val.clusterDim.y = 1;
-    attr[n].val.clusterDim.z = 1;
-    ++n;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = n;
-  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-}
 
 }  // namespace pn

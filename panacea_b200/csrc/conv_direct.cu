@@ -34,7 +34,6 @@ __global__ void __launch_bounds__(CD_THREADS) conv3x3_direct_kernel(const TIn* _
                                                                     float* __restrict__ y_f32, __nv_bfloat16* __restrict__ y_bf16,
                                                                     int F, int H, int W, int Cin, int Cout, int Cout_pad, int Ho,
                                                                     int Wo, int stride, int act_silu) {
-  pdl_prologue_done();
   extern __shared__ float sw[];  // [Cin][16]
   const int co0 = blockIdx.y * CD_COUT_TILE;
   const size_t pix = (size_t)blockIdx.x * CD_THREADS + threadIdx.x;
@@ -111,11 +110,11 @@ extern "C" int pn_conv3x3_direct(const void* x, int x_is_bf16, const float* w_pa
   PN_REQUIRE(smem <= 48 * 1024, "pn_conv3x3_direct: Cin=%lld too large for the direct path", (long long)Cin);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   if (x_is_bf16)
-    launch_kernel(conv3x3_direct_kernel<__nv_bfloat16>, dim3(grid), dim3(CD_THREADS), smem, st, 1, 
+    conv3x3_direct_kernel<__nv_bfloat16><<<grid, CD_THREADS, smem, st>>>(
         reinterpret_cast<const __nv_bfloat16*>(x), w_packed, bias, addend, y_f32, reinterpret_cast<__nv_bfloat16*>(y_bf16),
         (int)frames, (int)H, (int)W, (int)Cin, (int)Cout, (int)Cout_pad, Ho, Wo, stride, act_silu);
   else
-    launch_kernel(conv3x3_direct_kernel<float>, dim3(grid), dim3(CD_THREADS), smem, st, 1, 
+    conv3x3_direct_kernel<float><<<grid, CD_THREADS, smem, st>>>(
         reinterpret_cast<const float*>(x), w_packed, bias, addend, y_f32, reinterpret_cast<__nv_bfloat16*>(y_bf16),
         (int)frames, (int)H, (int)W, (int)Cin, (int)Cout, (int)Cout_pad, Ho, Wo, stride, act_silu);
   PN_CHECK_CUDA(cudaGetLastError());

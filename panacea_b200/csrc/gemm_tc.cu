@@ -105,7 +105,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_prologue_done();        // barriers are set up: from here on global memory is touched
 
   // The next k-block to load -> (tap row, tap column, 64-channel chunk), channel chunk fastest, advanced one k-block at
   // a time. Every thread keeps it, so thread 0's loads are issued by predicate, not by branch.
@@ -302,7 +301,8 @@ static int launch_gemm(const GemmParams& p, int mode, long long tiles, cudaStrea
                                                                                    : gemm_tc_kernel<BN, STAGES, 0>;
   const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), S::TOTAL, /*max_carveout=*/true);
   if (rc != PN_OK) return rc;
-  PN_CHECK_CUDA(launch_kernel(kern, dim3((unsigned)tiles), dim3(GEMM_THREADS), S::TOTAL, stream, 1, p));
+  kern<<<(unsigned)tiles, GEMM_THREADS, S::TOTAL, stream>>>(p);
+  PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
 

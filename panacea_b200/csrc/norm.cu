@@ -199,7 +199,6 @@ template <int CPG, int OP>
 __global__ void __launch_bounds__(512) gn_pixel_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
                                                        const float* __restrict__ beta, void* __restrict__ y,
                                                        int T, int P, int C, float eps, int act_silu) {
-  pdl_prologue_done();
   __shared__ float red[16][32];
   const int t = threadIdx.x >> 5, g = threadIdx.x & 31;
   const int b = blockIdx.x / P, p = blockIdx.x - b * P;
@@ -261,7 +260,6 @@ template <int MAXV, int OP, typename TIn>
 __global__ void __launch_bounds__(256) layernorm_kernel(const TIn* __restrict__ x, const float* __restrict__ gamma,
                                                         const float* __restrict__ beta, void* __restrict__ y,
                                                         long long rows, int C, float eps) {
-  pdl_prologue_done();
   const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
@@ -317,7 +315,6 @@ template <int LPR, int NV>
 __global__ void __launch_bounds__(256) layernorm_bf16_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma,
                                                              const float* __restrict__ beta, __nv_bfloat16* __restrict__ y,
                                                              long long rows, int C, float eps) {
-  pdl_prologue_done();
   constexpr int RPW = 32 / LPR;                                  // rows per warp and pass
   const int lane = threadIdx.x & 31, sub = lane % LPR;
   // the affine parameters are staged in shared memory once per CTA (re-reading them from global per row cost four times
@@ -382,8 +379,7 @@ using namespace pn;
 // wave = frames processed concurrently (their input fits L2), cpf = CTAs per frame; wave * cpf <= SM count
 static void gn_geometry(int64_t frames, int64_t pixels, int64_t channels, int* wave, int* cpf) {
   const size_t frame_bytes = (size_t)pixels * channels * sizeof(float);
-  static const size_t wave_bytes = [] { const char* e = std::getenv("PN_GN_WAVE_MB"); return e ? (size_t)std::atoi(e) << 20 : GN_WAVE_BYTES; }();
-  int w = (int)(wave_bytes / (frame_bytes ? frame_bytes : 1));
+  int w = (int)(GN_WAVE_BYTES / (frame_bytes ? frame_bytes : 1));
   if (w < 1) w = 1;
   if (w > frames) w = (int)frames;
   const int sms = sm_count();
@@ -485,7 +481,7 @@ extern "C" int pn_groupnorm_pixel_silu(const float* x, const float* gamma, const
   const int threads = (int)frames_per_seq * 32;
   const int T = (int)frames_per_seq, P = (int)pixels, C = (int)channels;
   switch (C / 32) {
-#define PN_GNP_CASE(CPG) case CPG: PN_DISPATCH_OP(operand_mode, (launch_kernel(gn_pixel_kernel<CPG, OP>, dim3((unsigned)blocks), dim3(threads), 0, st, 1, x, gamma, beta, y, T, P, C, eps, act_silu))); break;
+#define PN_GNP_CASE(CPG) case CPG: PN_DISPATCH_OP(operand_mode, gn_pixel_kernel<CPG, OP><<<(unsigned)blocks, threads, 0, st>>>(x, gamma, beta, y, T, P, C, eps, act_silu)); break;
     PN_GNP_CASE(2) PN_GNP_CASE(4) PN_GNP_CASE(6) PN_GNP_CASE(8) PN_GNP_CASE(10) PN_GNP_CASE(12) PN_GNP_CASE(16) PN_GNP_CASE(20)
     PN_GNP_CASE(24) PN_GNP_CASE(30) PN_GNP_CASE(32) PN_GNP_CASE(40) PN_GNP_CASE(60) PN_GNP_CASE(80)
 #undef PN_GNP_CASE
@@ -508,14 +504,14 @@ extern "C" int pn_layernorm(const void* x, int x_is_bf16, const float* gamma, co
   if (x_is_bf16 && operand_mode == PN_OP_BF16 && C % 64 == 0) {
     // fast path: LPR lanes per row, NV = C / (8 LPR) loads per lane (5 for C = 320 / 640 / 1280)
 #define PN_LNB(LPR, NV)                                                                                                            \
-    do {                                                                                                                            \
-      const long long rows_per_block = 8 * (32 / LPR);                                                                              \
-      long long nb = (rows + rows_per_block - 1) / rows_per_block;                                                                  \
+    do {                                                                                                                           \
+      const long long rows_per_block = 8 * (32 / LPR);                                                                             \
+      long long nb = (rows + rows_per_block - 1) / rows_per_block;                                                                 \
       if (nb > 6ll * sm_count()) nb = 6ll * sm_count();          /* grid-stride over the rows: affine parameters staged once per CTA */ \
-      launch_kernel(layernorm_bf16_kernel<LPR, NV>, dim3((unsigned)nb), dim3(256), (size_t)C * 8, st, 1, reinterpret_cast<const __nv_bfloat16*>(x), \
-                    gamma, beta, reinterpret_cast<__nv_bfloat16*>(y), (long long)rows, C, eps);                                     \
-      PN_CHECK_CUDA(cudaGetLastError());                                                                                            \
-      return PN_OK;                                                                                                                 \
+      layernorm_bf16_kernel<LPR, NV><<<(unsigned)nb, 256, (size_t)C * 8, st>>>(reinterpret_cast<const __nv_bfloat16*>(x),          \
+          gamma, beta, reinterpret_cast<__nv_bfloat16*>(y), (long long)rows, C, eps);                                              \
+      PN_CHECK_CUDA(cudaGetLastError());                                                                                           \
+      return PN_OK;                                                                                                                \
     } while (0)
     for (int lpr = 8; lpr <= 32; lpr *= 2) {
       if (C % (8 * lpr) != 0) continue;
@@ -529,13 +525,13 @@ extern "C" int pn_layernorm(const void* x, int x_is_bf16, const float* gamma, co
   }
   const long long blocks = (rows * 32 + 255) / 256;
 #define PN_LN(MAXV)                                                                                                          \
-  do {                                                                                                                      \
-    if (x_is_bf16)                                                                                                          \
-      PN_DISPATCH_OP(operand_mode, (launch_kernel(layernorm_kernel<MAXV, OP, __nv_bfloat16>, dim3((unsigned)blocks), dim3(256), 0, st, 1,              \
-                                       reinterpret_cast<const __nv_bfloat16*>(x), gamma, beta, y, rows, C, eps)));           \
-    else                                                                                                                    \
-      PN_DISPATCH_OP(operand_mode, (launch_kernel(layernorm_kernel<MAXV, OP, float>, dim3((unsigned)blocks), dim3(256), 0, st, 1,                      \
-                                       reinterpret_cast<const float*>(x), gamma, beta, y, rows, C, eps)));                   \
+  do {                                                                                                                       \
+    if (x_is_bf16)                                                                                                           \
+      PN_DISPATCH_OP(operand_mode, layernorm_kernel<MAXV, OP, __nv_bfloat16><<<(unsigned)blocks, 256, 0, st>>>(              \
+          reinterpret_cast<const __nv_bfloat16*>(x), gamma, beta, y, rows, C, eps));                                         \
+    else                                                                                                                     \
+      PN_DISPATCH_OP(operand_mode, layernorm_kernel<MAXV, OP, float><<<(unsigned)blocks, 256, 0, st>>>(                      \
+          reinterpret_cast<const float*>(x), gamma, beta, y, rows, C, eps));                                                 \
   } while (0)
   if (C <= 512) PN_LN(4);
   else if (C <= 1024) PN_LN(8);

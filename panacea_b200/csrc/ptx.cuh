@@ -26,17 +26,6 @@ __device__ __forceinline__ bool elect_one() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// Programmatic dependent launch: every kernel of the step is launched with programmatic stream serialization
-// (common.cuh::launch_kernel). `pdl_prologue_done()` lets the NEXT kernel's CTAs be scheduled as this kernel's CTAs
-// retire (its launch latency, barrier/TMEM set-up and the tail of this grid overlap) and then blocks until every
-// prerequisite grid has completed and flushed its memory; nothing before it may touch global memory.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void pdl_prologue_done() {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
 // mbarrier
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {

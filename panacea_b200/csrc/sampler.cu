@@ -2,10 +2,7 @@
 // evaluation into the next sampler state and the next network input. It restates, in the reference's fp32 operation
 // order, the denoiser scalings (denoiser.py:22-28 with EpsScaling), the guidance combine (guiders.py:25-29,
 // sampling_utils.py:7-9) and the solver updates of sampling.py:85-365 (see pn_sampler_mode in the header).
-#include <cstring>
-
 #include "common.cuh"
-#include "ptx.cuh"
 #include "../../include/panacea_b200.h"
 
 namespace pn {
@@ -50,7 +47,6 @@ __device__ __forceinline__ float philox_normal(uint64_t seed, uint64_t draw, uin
 // ---------------------------------------------------------------- the step kernel
 template <int MODE>
 __global__ void sampler_step_kernel(pn_sampler_step_args a) {
-  pdl_prologue_done();
   const size_t n = (size_t)a.n;
   float* out = a.out ? a.out : a.x;
   for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x) {
@@ -102,14 +98,6 @@ __global__ void sampler_step_kernel(pn_sampler_step_args a) {
   }
 }
 
-static inline int step_grid(size_t total, int threads = 256) {
-  size_t g = (total + threads - 1) / threads;
-  const size_t cap = (size_t)16 * sm_count();
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
 }  // namespace pn
 
 using namespace pn;
@@ -127,31 +115,16 @@ extern "C" int pn_sampler_step(const pn_sampler_step_args* a, void* stream_v) {
   PN_REQUIRE(!(reads_hist || a->hist_write >= 0) || a->hist, "pn_sampler_step: hist is NULL");
   PN_REQUIRE(!reads_hist || a->mode == PN_SAMPLER_LMS || a->hist_read[0] >= 0, "pn_sampler_step: hist_read[0] missing");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  const dim3 grid(step_grid((size_t)a->n)), block(256);
+  const dim3 grid(stride_grid((size_t)a->n)), block(256);
   switch (a->mode) {
-    case PN_SAMPLER_EULER: launch_kernel(sampler_step_kernel<PN_SAMPLER_EULER>, grid, block, 0, st, 1, *a); break;
-    case PN_SAMPLER_HEUN: launch_kernel(sampler_step_kernel<PN_SAMPLER_HEUN>, grid, block, 0, st, 1, *a); break;
-    case PN_SAMPLER_LMS: launch_kernel(sampler_step_kernel<PN_SAMPLER_LMS>, grid, block, 0, st, 1, *a); break;
-    case PN_SAMPLER_DPM: launch_kernel(sampler_step_kernel<PN_SAMPLER_DPM>, grid, block, 0, st, 1, *a); break;
-    case PN_SAMPLER_DPM_2M: launch_kernel(sampler_step_kernel<PN_SAMPLER_DPM_2M>, grid, block, 0, st, 1, *a); break;
-    default: launch_kernel(sampler_step_kernel<PN_SAMPLER_SCALE>, grid, block, 0, st, 1, *a); break;
+    case PN_SAMPLER_EULER: sampler_step_kernel<PN_SAMPLER_EULER><<<grid, block, 0, st>>>(*a); break;
+    case PN_SAMPLER_HEUN: sampler_step_kernel<PN_SAMPLER_HEUN><<<grid, block, 0, st>>>(*a); break;
+    case PN_SAMPLER_LMS: sampler_step_kernel<PN_SAMPLER_LMS><<<grid, block, 0, st>>>(*a); break;
+    case PN_SAMPLER_DPM: sampler_step_kernel<PN_SAMPLER_DPM><<<grid, block, 0, st>>>(*a); break;
+    case PN_SAMPLER_DPM_2M: sampler_step_kernel<PN_SAMPLER_DPM_2M><<<grid, block, 0, st>>>(*a); break;
+    default: sampler_step_kernel<PN_SAMPLER_SCALE><<<grid, block, 0, st>>>(*a); break;
   }
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
 
-// The Euler + CFG step of EulerEDMSampler (s_churn = 0): PN_SAMPLER_EULER with two halves, in place.
-extern "C" int pn_cfg_euler_step(float* x, const float* net2, float* x_in_next, int64_t n, float sigma, float sigma_q,
-                                 float sigma_next, float cfg_scale, float c_in_next, int net_is_denoised,
-                                 void* stream_v) {
-  PN_REQUIRE(x && net2 && n > 0 && sigma > 0.f, "pn_cfg_euler_step: bad arguments");
-  pn_sampler_step_args a;
-  memset(&a, 0, sizeof(a));
-  a.x = x; a.net = net2; a.x_in_next = x_in_next; a.n = n;
-  a.mode = PN_SAMPLER_EULER; a.halves = 2; a.net_is_denoised = net_is_denoised;
-  a.hist_read[0] = a.hist_read[1] = a.hist_read[2] = -1; a.hist_write = -1;
-  a.sigma_q = sigma_q; a.cfg_scale = cfg_scale; a.sigma = sigma;
-  a.dt = sigma_next - sigma;
-  a.c_in_next = c_in_next;
-  return pn_sampler_step(&a, stream_v);
-}

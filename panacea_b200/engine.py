@@ -17,8 +17,6 @@ from __future__ import annotations
 
 import math
 
-import os
-
 import torch
 
 from .ops import geglu_pack
@@ -81,7 +79,7 @@ class Engine:
         self.generation = 0
         self.cond = {"guided": None, "kv": {}, "b": None}     # step-invariant state (prepare_hint / prepare_text)
         self._xin = {}
-        self.two_streams = os.environ.get("PN_TWO_STREAMS", "1") != "0"      # ControlNet || UNet encoder (see eps)
+        self.two_streams = True         # ControlNet || UNet encoder (see eps); False gives the single-stream launch order
         self._side = None
 
     # ------------------------------------------------------------------------------------------ packing
@@ -478,7 +476,7 @@ class Engine:
             # everything else). The big level-0/1 launches have many waves of tiles and fill all SMs either way; what
             # overlaps is the under-filled tail — level-2/3/mid GEMMs and attentions with fewer tiles than SMs, small
             # norms — and, since the GEMM kernel fits two CTAs per SM, a GEMM tile of one branch can share an SM with a
-            # tile of the other. PN_TWO_STREAMS=0 restores the single-stream order.
+            # tile of the other.
             cur = torch.cuda.current_stream(xin.device)
             if self._side is None or self._side.device != xin.device:
                 self._side = torch.cuda.Stream(device=xin.device)

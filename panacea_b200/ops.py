@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -53,6 +54,24 @@ def split3(t: torch.Tensor, taps: int = 1) -> torch.Tensor:
     return torch.cat([hi, hi, lo], dim=2).reshape(n, 3 * k).contiguous()
 
 
+def _attn_args(q, k, v, out, *, q_ld, kv_ld, F, H, V, W, Hk, Vk, Wk, heads, head_dim, views):
+    """pn_attn_args for pn_attention / pn_attention_f32: q, k, v, out are device addresses, the output dense
+    ([tokens, heads * head_dim]); query view v attends the key views views[v]."""
+    a = _lib.AttnArgs()
+    a.q, a.k, a.v, a.out = q, k, v, out
+    a.q_ld, a.kv_ld, a.out_ld = q_ld, kv_ld, heads * head_dim
+    a.F, a.H, a.V, a.W = F, H, V, W
+    a.Hk, a.Vk, a.Wk = Hk, Vk, Wk
+    a.kv_frame_div = 1
+    a.heads, a.head_dim = heads, head_dim
+    for vi, lst in enumerate(views):
+        a.kv_view_count[vi] = len(lst)
+        for j, kvv in enumerate(lst):
+            a.kv_views[vi][j] = kvv
+    a.scale = head_dim ** -0.5
+    return a
+
+
 class NativeOps:
     """The production op set (bf16 operands). `launches` counts kernel launches issued through the C ABI.
     `operand_mode` / `operand_mult` describe how producers store GEMM operands (ParityOps overrides them)."""
@@ -67,14 +86,9 @@ class NativeOps:
     LN_FOLD_MAX_C = 640       # LayerNorm fold up to C = 640; wider token streams keep the LayerNorm kernel
 
     def __init__(self):
-        import os
         self.lib = _lib.load()
         self.launches = 0
         self._freqs = {}
-        if os.environ.get("PN_TOKEN_F32") == "1" and self.operand_mode == OP_BF16:      # A/B measurement of the bf16 token stream
-            self.token_dtype = F32
-        if os.environ.get("PN_LN_FOLD") == "0" or self.token_dtype != BF16:              # A/B measurement of the LayerNorm fold
-            self.fold_layernorm = False
 
     def pack_matrix(self, w: torch.Tensor, taps: int = 1) -> torch.Tensor:
         """fp32 weight [N, taps*C] -> the B operand pn_gemm reads in this op set's precision mode."""
@@ -230,20 +244,8 @@ class NativeOps:
         return y
 
     # ------------------------------------------------------------------ attention
-    def _attention(self, q, k, v, out, *, q_ld, kv_ld, out_ld, F, H, V, W, Hk, Vk, Wk, kv_frame_div, heads, views, head_dim=64):
-        a = _lib.AttnArgs()
-        a.q, a.k, a.v, a.out = q, k, v, out
-        a.q_ld, a.kv_ld, a.out_ld = q_ld, kv_ld, out_ld
-        a.F, a.H, a.V, a.W = F, H, V, W
-        a.Hk, a.Vk, a.Wk = Hk, Vk, Wk
-        a.kv_frame_div = kv_frame_div
-        a.heads, a.head_dim = heads, head_dim
-        for vi, lst in enumerate(views):
-            a.kv_view_count[vi] = len(lst)
-            for j, kvv in enumerate(lst):
-                a.kv_views[vi][j] = kvv
-        a.scale = head_dim ** -0.5
-        _lib.check(self.lib.pn_attention(C.byref(a), _stream()), "pn_attention")
+    def _attention(self, q, k, v, out, **geometry):
+        _lib.check(self.lib.pn_attention(C.byref(_attn_args(q, k, v, out, **geometry)), _stream()), "pn_attention")
         self.launches += 1
 
     def attention_view(self, qkv, heads, cross, neighbours):
@@ -257,8 +259,8 @@ class NativeOps:
         out = torch.empty((Fr, H, V, w, Cc), device=qkv.device, dtype=BF16)
         views = [list(neighbours[v]) for v in range(V)] if cross else [[v] for v in range(V)]
         base = qkv.data_ptr()
-        self._attention(base, base + 2 * Cc, base + 4 * Cc, out.data_ptr(), q_ld=C3, kv_ld=C3, out_ld=Cc, F=Fr, H=H, V=V, W=w,
-                        Hk=H, Vk=V, Wk=w, kv_frame_div=1, heads=heads, views=views, head_dim=d)
+        self._attention(base, base + 2 * Cc, base + 4 * Cc, out.data_ptr(), q_ld=C3, kv_ld=C3, F=Fr, H=H, V=V, W=w, Hk=H, Vk=V, Wk=w,
+                        heads=heads, head_dim=d, views=views)
         return out
 
     def attention_text(self, q, kv, heads):
@@ -271,8 +273,8 @@ class NativeOps:
              "attention_text: bad shapes")
         out = torch.empty_like(q)
         base = kv.data_ptr()
-        self._attention(q.data_ptr(), base, base + 2 * Cc, out.data_ptr(), q_ld=Cc, kv_ld=2 * Cc, out_ld=Cc, F=b, H=1, V=1,
-                        W=Nq, Hk=1, Vk=1, Wk=Nk, kv_frame_div=1, heads=heads, views=[[0]], head_dim=d)
+        self._attention(q.data_ptr(), base, base + 2 * Cc, out.data_ptr(), q_ld=Cc, kv_ld=2 * Cc, F=b, H=1, V=1, W=Nq, Hk=1, Vk=1,
+                        Wk=Nk, heads=heads, head_dim=d, views=[[0]])
         return out
 
     def attention_temporal(self, qkv, heads):
@@ -439,12 +441,9 @@ class NativeOps:
     def cfg_euler_step(self, x, net2, x_in_next, sigma, sigma_next, scale, c_in_next, sigma_q=None, net_is_denoised=False):
         _req(x.dtype == F32 and net2.dtype == F32 and x.is_contiguous() and net2.is_contiguous() and net2.numel() == 2 * x.numel(),
              "cfg_euler_step: shapes")
-        sq = sigma if sigma_q is None else sigma_q
-        _lib.check(self.lib.pn_cfg_euler_step(_ptr(x), _ptr(net2), _ptr(x_in_next), x.numel(), float(sigma), float(sq),
-                                             float(sigma_next), float(scale), float(c_in_next), int(bool(net_is_denoised)),
-                                             _stream()), "pn_cfg_euler_step")
-        self.launches += 1
-        return x
+        dt = float(np.float32(sigma_next) - np.float32(sigma))       # the fp32 difference of the fp32 sigmas
+        return self.sampler_step(SAMPLER_EULER, x, net2, x_in_next=x_in_next, sigma_q=sigma if sigma_q is None else sigma_q,
+                                 cfg_scale=scale, sigma=sigma, dt=dt, c_in_next=c_in_next, net_is_denoised=net_is_denoised)
 
     def sampler_step(self, mode, x, net=None, *, x_eval=None, out=None, hist=None, noise=None, x_in_next=None, halves=2,
                      net_is_denoised=False, sigma_q=0.0, cfg_scale=1.0, sigma=0.0, dt=0.0, coef=(), hist_read=(),
@@ -479,11 +478,12 @@ class NativeOps:
         return x if out is None else out
 
     def softmax_rows(self, s, scale):
-        """fp32 [rows, N] -> bf16 [rows, N] = softmax(scale * s) per row (VAE mid-block attention)."""
+        """fp32 [rows, N] -> softmax(scale * s) per row as the operand of the O = P v GEMM (VAE mid-block attention): bf16
+        [rows, N], or in parity mode the split3 operand bf16 [rows, 3N] = [hi | lo | hi]."""
         _req(s.is_cuda and s.dtype == F32 and s.dim() == 2 and s.is_contiguous() and s.shape[1] % 4 == 0, "softmax_rows: fp32 [rows, N]")
-        out = torch.empty(s.shape, device=s.device, dtype=BF16)
-        _lib.check(self.lib.pn_softmax_rows(_ptr(s), _ptr(out), s.shape[0], s.shape[1], s.stride(0), out.stride(0), float(scale),
-                                           _stream()), "pn_softmax_rows")
+        out = self._operand_empty(s.shape, s.device)
+        _lib.check(self.lib.pn_softmax_rows_operand(_ptr(s), _ptr(out), s.shape[0], s.shape[1], s.stride(0), out.stride(0), float(scale),
+                                                   self.operand_mode, _stream()), "pn_softmax_rows_operand")
         self.launches += 1
         return out
 
@@ -539,30 +539,10 @@ class ParityOps(NativeOps):
         _req(out_dtype == F32, "parity gemm: outputs are fp32 (operands are produced by cast_operand)")
         return super().gemm(a, w, out_dtype=F32, **kw)
 
-    def softmax_rows(self, s, scale):
-        """fp32 [rows, N] -> split3 operand bf16 [rows, 3N] = [hi | lo | hi] of softmax(scale * s) per row."""
-        _req(s.is_cuda and s.dtype == F32 and s.dim() == 2 and s.is_contiguous() and s.shape[1] % 4 == 0, "softmax_rows: fp32 [rows, N]")
-        out = self._operand_empty(s.shape, s.device)
-        _lib.check(self.lib.pn_softmax_rows_operand(_ptr(s), _ptr(out), s.shape[0], s.shape[1], s.stride(0), out.stride(0), float(scale),
-                                                   self.operand_mode, _stream()), "pn_softmax_rows_operand")
-        self.launches += 1
-        return out
-
     # ------------------------------------------------------------------ attention (fp32, CUDA cores)
-    def _attention_f32(self, q, k, v, out, *, q_ld, kv_ld, F, H, V, W, Hk, Vk, Wk, heads, head_dim, views):
-        a = _lib.AttnArgs()
-        a.q, a.k, a.v, a.out = q, k, v, out
-        a.q_ld, a.kv_ld, a.out_ld = q_ld, kv_ld, heads * head_dim
-        a.F, a.H, a.V, a.W = F, H, V, W
-        a.Hk, a.Vk, a.Wk = Hk, Vk, Wk
-        a.kv_frame_div = 1
-        a.heads, a.head_dim = heads, head_dim
-        for vi, lst in enumerate(views):
-            a.kv_view_count[vi] = len(lst)
-            for j, kvv in enumerate(lst):
-                a.kv_views[vi][j] = kvv
-        a.scale = head_dim ** -0.5
-        _lib.check(self.lib.pn_attention_f32(C.byref(a), self.operand_mode, _stream()), "pn_attention_f32")
+    def _attention_f32(self, q, k, v, out, **geometry):
+        _lib.check(self.lib.pn_attention_f32(C.byref(_attn_args(q, k, v, out, **geometry)), self.operand_mode, _stream()),
+                   "pn_attention_f32")
         self.launches += 1
 
     def attention_view(self, qkv, heads, cross, neighbours):

@@ -7,7 +7,7 @@ AttnBlock / ResnetBlock, then per level 3 ResnetBlocks (+ nearest-2x Upsample + 
 + conv_out) on channels-last buffers over the 6-view panorama, with the kernels of the UNet path: `pn_gemm` for every
 3x3 / 1x1 convolution (residual and shortcut adds in the epilogue), `pn_groupnorm_silu`, `pn_upsample2x`,
 `pn_conv3x3_direct` for the 4-channel input and 3-channel output convs, and — for the single-head attention of the mid
-block whose head_dim is the full channel count (512) — two GEMMs around `pn_softmax_rows` per frame:
+block whose head_dim is the full channel count (512) — two GEMMs around `pn_softmax_rows_operand` per frame:
 S = q k^T, P = softmax(S / sqrt(C)), O = P v (the value bias is added after the product: rows of P sum to one).
 The op set decides the precision, as on the UNet: NativeOps gives bf16 operands with fp32 accumulation and residual
 stream; ParityOps gives split-bf16 operands (fp32-class products), the reference's fp32 VAE to rtol 1e-3 / atol 1e-4.

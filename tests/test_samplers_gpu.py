@@ -95,7 +95,8 @@ def test_sampler_step_kernel_matches_torch(ops, mode, halves, noise):
 
 
 def test_net_is_denoised_and_euler_wrapper(ops):
-    """pn_cfg_euler_step is PN_SAMPLER_EULER with two halves (bit-identical), and net_is_denoised skips the scalings."""
+    """cfg_euler_step is PN_SAMPLER_EULER with two halves and dt rounded in fp32 (bit-identical), and net_is_denoised skips
+    the scalings."""
     x = _rand(SHAPE, 11, 10.0)
     net = _rand((16,) + SHAPE[1:], 12)
     a, b = x.clone(), x.clone()

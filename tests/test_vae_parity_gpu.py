@@ -58,7 +58,7 @@ def test_softmax_rows_operand(rows, N):
     ref_bf16 = ops.softmax_rows(s, scale)
     got_bf16 = torch.empty_like(ref_bf16)
     assert _softmax_operand(ops.lib, s, OP_BF16, got_bf16, scale) == 0
-    assert torch.equal(got_bf16, ref_bf16), "bf16 mode must be bitwise pn_softmax_rows"
+    assert torch.equal(got_bf16, ref_bf16), "bf16 mode must be bitwise NativeOps.softmax_rows"
     p3 = pops.softmax_rows(s, scale)
     assert p3.shape == (rows, 3 * N) and p3.dtype == torch.bfloat16
     hi, lo, hi2 = p3.float().split(N, dim=-1)

@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define PN_ABI_VERSION 3
+#define PN_ABI_VERSION 4
 
 enum pn_status { PN_STATUS_OK = 0, PN_STATUS_INVALID = -1, PN_STATUS_CUDA = -2, PN_STATUS_UNSUPPORTED = -3 };
 
@@ -96,7 +96,14 @@ int pn_gemm(const pn_gemm_args* args, void* stream);
 int pn_gemm_ln_parts(int N);
 
 /* ------------------------------------------------------------------------------------------------
- * pn_attention — wgmma flash attention over view-tiled tokens (head_dim 64).
+ * Attention. Each entry point serves both precision modes through its operand_mode:
+ *  PN_OPERAND_BF16                    q/k/v/out bf16, tensor-core kernels (fp32 softmax), strides in bf16 elements;
+ *  PN_OPERAND_SPLIT3 / PN_OPERAND_F32 parity mode: q/k/v fp32 (strides in floats, multiples of 4), fp32 products,
+ *                                     softmax and accumulation on CUDA cores; `out` is the dense operand of the to_out
+ *                                     GEMM [tokens, heads*head_dim] in that mode, so out_ld must equal heads*head_dim.
+ * Any other mode returns PN_STATUS_INVALID.
+ *
+ * pn_attention — flash attention over view-tiled tokens (head_dim 64 or 80; bf16: wgmma).
  * Replaces: xformers.ops.memory_efficient_attention inside MemoryEfficientIntraViewAttention.forward
  * (attention.py:407-489) and MemoryEfficientInterViewAttentionTwo.forward (attention.py:518-610), and
  * F.scaled_dot_product_attention inside CrossAttention.forward for the 77-token text context
@@ -105,13 +112,13 @@ int pn_gemm_ln_parts(int N);
  * attends the key views kv_views[v][0 .. kv_view_count[v]) (all rows/columns of those views):
  *   intra-view : kv_views[v] = {v};   cross-view : the reference's table {5,1},{0,2},{1,3},{2,4},{3,5},{4};
  *   text       : V = Vk = 1, W = tokens per batch element, Wk = 77, kv_views[0] = {0}.
- * out[token, head*64 + d] = softmax(q k^T * scale) v, bf16, token stride out_ld.
+ * out[token, head*head_dim + d] = softmax(q k^T * scale) v, token stride out_ld.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct pn_attn_args {
-  const void* q;   /* bf16, channel 0 of head 0 of the first query token */
-  const void* k;   /* bf16, likewise for keys (may point into the same fused qkv buffer) */
+  const void* q;   /* channel 0 of head 0 of the first query token */
+  const void* k;   /* likewise for keys (may point into the same fused qkv buffer) */
   const void* v;
-  void* out;       /* bf16 */
+  void* out;
   int64_t q_ld, kv_ld, out_ld;
   int64_t F, H, V, W;
   int64_t Hk, Vk, Wk;
@@ -122,33 +129,21 @@ typedef struct pn_attn_args {
   float scale;
 } pn_attn_args;
 
-int pn_attention(const pn_attn_args* args, void* stream);
+int pn_attention(const pn_attn_args* args, int operand_mode, void* stream);
 
 /* Temporal self-attention over T <= 16 frames per pixel (attention.py:1116-1125 -> :229-291, context=None).
- * q/k/v/out bf16 [batch, T, pixels, ld]; one (batch, pixel, head) sequence per warp (warp-level bf16 MMAs, fp32
- * softmax); ld and out_ld multiples of 8. */
+ * q/k/v [batch, T, pixels, ld], out [batch, T, pixels, out_ld]; head_dim 64 or 80. bf16: one (batch, pixel, head)
+ * sequence per warp (warp-level bf16 MMAs, fp32 softmax), ld and out_ld multiples of 8. */
 int pn_attention_temporal(const void* q, const void* k, const void* v, void* out, int64_t batch, int64_t T,
                           int64_t pixels, int32_t heads, int32_t head_dim, int64_t ld, int64_t out_ld, float scale,
-                          void* stream);
-
-/* Parity-mode attention: the same geometry (pn_attn_args; q/k/v are fp32 here, strides in floats, out_ld must be
- * heads*head_dim), fp32 products / softmax / accumulation on CUDA cores, head_dim 64 or 80; `out` is written as the
- * operand of the to_out GEMM in `operand_mode`. Same reference call sites as pn_attention / pn_attention_temporal. */
-int pn_attention_f32(const pn_attn_args* args, int operand_mode, void* stream);
-int pn_attention_temporal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t T,
-                              int64_t pixels, int32_t heads, int32_t head_dim, int64_t ld, float scale, int operand_mode,
-                              void* stream);
+                          int operand_mode, void* stream);
 
 /* Causal self-attention of the OpenCLIP text transformer (reference sgm/modules/encoders/modules.py:618-629, each
  * resblock's nn.MultiheadAttention with attn_mask = -inf above the diagonal: token i attends keys j <= i).
- * q/k/v bf16 [batch, L, ld] (e.g. three base pointers into the fused in_proj output), out bf16 [batch, L, out_ld];
- * L <= 128, head_dim 64, ld and out_ld multiples of 8. One CTA per (batch, head), warp-level bf16 MMAs, fp32 softmax. */
+ * q/k/v [batch, L, ld] (e.g. three base pointers into the fused in_proj output), out [batch, L, out_ld]; L <= 128,
+ * head_dim 64. bf16: one CTA per (batch, head), warp-level bf16 MMAs, fp32 softmax, ld and out_ld multiples of 8. */
 int pn_attention_causal(const void* q, const void* k, const void* v, void* out, int64_t batch, int64_t L, int32_t heads,
-                        int32_t head_dim, int64_t ld, int64_t out_ld, float scale, void* stream);
-/* Parity-mode twin of pn_attention_causal (same call site): q/k/v fp32 [batch, L, ld], fp32 math on CUDA cores, `out`
- * written as the out_proj GEMM operand [batch*L, heads*64] in `operand_mode`. */
-int pn_attention_causal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t L,
-                            int32_t heads, int32_t head_dim, int64_t ld, float scale, int operand_mode, void* stream);
+                        int32_t head_dim, int64_t ld, int64_t out_ld, float scale, int operand_mode, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Normalisation (fp32 residual stream in, bf16 MMA operand out)
@@ -176,7 +171,7 @@ int pn_layernorm(const void* x, int x_is_bf16, const float* gamma, const float* 
                  int64_t channels, float eps, int operand_mode, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Convolutions that cannot feed a 64-wide UMMA K block, layout and sampler helpers
+ * Convolutions that cannot feed a 64-wide wgmma K block, layout and sampler helpers
  * ---------------------------------------------------------------------------------------------- */
 /* Direct 3x3 conv, pad 1, stride 1|2, channels-last (stem openaimodel.py:977, head :1251, BEV hint stem
  * controlmodel.py:43-59). w_packed fp32 [9][Cin][Cout_pad]; y = act(conv + bias) + addend. */

@@ -66,12 +66,9 @@ SIGNATURES: dict[str, tuple] = {
     "pn_abi_version": (C.c_int, []),
     "pn_gemm": (C.c_int, [C.POINTER(GemmArgs), C.c_void_p]),
     "pn_gemm_ln_parts": (C.c_int, [C.c_int]),
-    "pn_attention": (C.c_int, [C.POINTER(AttnArgs), _vp]),
-    "pn_attention_temporal": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i64, _i64, _f32, _vp]),
-    "pn_attention_f32": (C.c_int, [C.POINTER(AttnArgs), C.c_int, _vp]),
-    "pn_attention_temporal_f32": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i64, _f32, C.c_int, _vp]),
-    "pn_attention_causal": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i64, _i64, _f32, _vp]),
-    "pn_attention_causal_f32": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i64, _f32, C.c_int, _vp]),
+    "pn_attention": (C.c_int, [C.POINTER(AttnArgs), C.c_int, _vp]),
+    "pn_attention_temporal": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i64, _i64, _f32, C.c_int, _vp]),
+    "pn_attention_causal": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i64, _i64, _f32, C.c_int, _vp]),
     "pn_groupnorm_workspace_floats": (_i64, [_i64, _i64, _i64]),
     "pn_groupnorm_ctas_per_frame": (_i64, [_i64, _i64, _i64]),
     "pn_groupnorm_silu": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _f32, C.c_int, C.c_int, _vp]),

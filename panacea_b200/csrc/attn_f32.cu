@@ -1,6 +1,6 @@
 // fp32 attention on CUDA cores — the attention of the PARITY mode (fp32-class arithmetic end to end, see operand.cuh).
 //
-// Same token geometry and view tables as the tcgen05 kernel (attn_fa.cu, pn_attn_args), but q/k/v are fp32, the
+// Same token geometry and view tables as the wgmma kernel (attn_fa.cu, pn_attn_args), but q/k/v are fp32, the
 // products, the softmax (exp2f, not the MUFU approximation) and the PV accumulation are fp32 FMAs, and the output is
 // written as the operand of the to_out GEMM (split3 in parity mode). It also covers head_dim 80 (BASELINE config 5).
 // Throughput is irrelevant here (a full-size eps-eval spends ~30 ms in it); exactness against the reference's
@@ -232,21 +232,18 @@ __global__ void __launch_bounds__(128) attn_f32_causal_kernel(const float* __res
   }
 }
 
-}  // namespace pn
-
-using namespace pn;
-
-extern "C" int pn_attention_causal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t L,
-                                       int32_t heads, int32_t head_dim, int64_t ld, float scale, int operand_mode,
-                                       void* stream_v) {
-  PN_REQUIRE(q && k && v && out, "pn_attention_causal_f32: null pointer");
-  PN_REQUIRE(head_dim == 64, "pn_attention_causal_f32: head_dim %d unsupported (64)", head_dim);
-  PN_REQUIRE(batch > 0 && L >= 1 && L <= 128 && heads > 0, "pn_attention_causal_f32: bad geometry (1 <= L <= 128)");
-  PN_REQUIRE(ld % 4 == 0 && ld >= (int64_t)heads * head_dim, "pn_attention_causal_f32: bad token stride");
-  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_attention_causal_f32: operand_mode %d", operand_mode);
+// The parity-mode launchers behind pn_attention / pn_attention_temporal / pn_attention_causal (declared in common.cuh):
+// those entry points call them for operand_mode PN_OPERAND_SPLIT3 / PN_OPERAND_F32.
+int attention_causal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t L, int32_t heads,
+                         int32_t head_dim, int64_t ld, int64_t out_ld, float scale, int operand_mode, void* stream_v) {
+  PN_REQUIRE(q && k && v && out, "pn_attention_causal: null pointer");
+  PN_REQUIRE(head_dim == 64, "pn_attention_causal: head_dim %d unsupported (64)", head_dim);
+  PN_REQUIRE(batch > 0 && L >= 1 && L <= 128 && heads > 0, "pn_attention_causal: bad geometry (1 <= L <= 128)");
+  PN_REQUIRE(ld % 4 == 0 && ld >= (int64_t)heads * head_dim, "pn_attention_causal: bad token stride");
+  PN_REQUIRE(out_ld == (int64_t)heads * head_dim, "pn_attention_causal: out_ld must equal heads*head_dim (dense operand)");
   const long long total = batch * heads * L;
   const long long blocks = (total + 127) / 128;
-  PN_REQUIRE(blocks < (1ll << 31), "pn_attention_causal_f32: grid too large");
+  PN_REQUIRE(blocks < (1ll << 31), "pn_attention_causal: grid too large");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   PN_DISPATCH_OP(operand_mode, attn_f32_causal_kernel<OP><<<(unsigned)blocks, 128, 0, st>>>(q, k, v, out, (int)batch, (int)L, heads, ld,
                                                                                          scale * 1.4426950408889634f));
@@ -254,15 +251,14 @@ extern "C" int pn_attention_causal_f32(const float* q, const float* k, const flo
   return PN_OK;
 }
 
-extern "C" int pn_attention_f32(const pn_attn_args* a, int operand_mode, void* stream_v) {
-  if (a == nullptr) return fail(PN_ERR_INVALID, "pn_attention_f32: null args");
-  PN_REQUIRE(a->q && a->k && a->v && a->out, "pn_attention_f32: null tensor pointer");
-  PN_REQUIRE(a->head_dim == 64 || a->head_dim == 80, "pn_attention_f32: head_dim %d unsupported (64 or 80)", a->head_dim);
-  PN_REQUIRE(a->heads > 0 && a->F > 0 && a->H > 0 && a->V > 0 && a->V <= 8 && a->W > 0, "pn_attention_f32: bad query geometry");
-  PN_REQUIRE(a->Hk > 0 && a->Vk > 0 && a->Vk <= 8 && a->Wk > 0 && a->kv_frame_div > 0, "pn_attention_f32: bad key geometry");
-  PN_REQUIRE(a->q_ld % 4 == 0 && a->kv_ld % 4 == 0, "pn_attention_f32: token strides must be multiples of 4 floats");
-  PN_REQUIRE(a->out_ld == (int64_t)a->heads * a->head_dim, "pn_attention_f32: out_ld must equal heads*head_dim (dense operand)");
-  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_attention_f32: operand_mode %d", operand_mode);
+int attention_f32(const pn_attn_args* a, int operand_mode, void* stream_v) {
+  if (a == nullptr) return fail(PN_ERR_INVALID, "pn_attention: null args");
+  PN_REQUIRE(a->q && a->k && a->v && a->out, "pn_attention: null tensor pointer");
+  PN_REQUIRE(a->head_dim == 64 || a->head_dim == 80, "pn_attention: head_dim %d unsupported (64 or 80)", a->head_dim);
+  PN_REQUIRE(a->heads > 0 && a->F > 0 && a->H > 0 && a->V > 0 && a->V <= 8 && a->W > 0, "pn_attention: bad query geometry");
+  PN_REQUIRE(a->Hk > 0 && a->Vk > 0 && a->Vk <= 8 && a->Wk > 0 && a->kv_frame_div > 0, "pn_attention: bad key geometry");
+  PN_REQUIRE(a->q_ld % 4 == 0 && a->kv_ld % 4 == 0, "pn_attention: fp32 token strides must be multiples of 4 floats");
+  PN_REQUIRE(a->out_ld == (int64_t)a->heads * a->head_dim, "pn_attention: out_ld must equal heads*head_dim (dense operand)");
   AfParams p;
   std::memset(&p, 0, sizeof(p));
   p.q = reinterpret_cast<const float*>(a->q); p.k = reinterpret_cast<const float*>(a->k); p.v = reinterpret_cast<const float*>(a->v);
@@ -273,17 +269,17 @@ extern "C" int pn_attention_f32(const pn_attn_args* a, int operand_mode, void* s
   p.kv_frame_div = a->kv_frame_div; p.heads = a->heads;
   for (int v = 0; v < a->V; ++v) {
     const int cnt = a->kv_view_count[v];
-    PN_REQUIRE(cnt >= 1 && cnt <= 2, "pn_attention_f32: kv_view_count[%d]=%d must be 1 or 2", v, cnt);
+    PN_REQUIRE(cnt >= 1 && cnt <= 2, "pn_attention: kv_view_count[%d]=%d must be 1 or 2", v, cnt);
     p.kv_view_count[v] = cnt;
     for (int i = 0; i < cnt; ++i) {
-      PN_REQUIRE(a->kv_views[v][i] >= 0 && a->kv_views[v][i] < a->Vk, "pn_attention_f32: kv view out of range");
+      PN_REQUIRE(a->kv_views[v][i] >= 0 && a->kv_views[v][i] < a->Vk, "pn_attention: kv view out of range");
       p.kv_views[v][i] = a->kv_views[v][i];
     }
   }
   p.scale_log2 = a->scale * 1.4426950408889634f;
   const long long tiles = (a->H * a->W + AF_QTILE - 1) / AF_QTILE;
   const long long blocks = tiles * a->heads * a->V * a->F;
-  PN_REQUIRE(blocks > 0 && blocks < (1ll << 31), "pn_attention_f32: grid too large");
+  PN_REQUIRE(blocks > 0 && blocks < (1ll << 31), "pn_attention: grid too large");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   if (a->head_dim == 64) PN_DISPATCH_OP(operand_mode, attn_f32_view_kernel<64, OP><<<(unsigned)blocks, AF_QTILE, 0, st>>>(p));
   else PN_DISPATCH_OP(operand_mode, attn_f32_view_kernel<80, OP><<<(unsigned)blocks, AF_QTILE, 0, st>>>(p));
@@ -291,17 +287,17 @@ extern "C" int pn_attention_f32(const pn_attn_args* a, int operand_mode, void* s
   return PN_OK;
 }
 
-extern "C" int pn_attention_temporal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t T,
-                                         int64_t pixels, int32_t heads, int32_t head_dim, int64_t ld, float scale,
-                                         int operand_mode, void* stream_v) {
-  PN_REQUIRE(q && k && v && out, "pn_attention_temporal_f32: null pointer");
-  PN_REQUIRE(head_dim == 64 || head_dim == 80, "pn_attention_temporal_f32: head_dim %d unsupported (64 or 80)", head_dim);
-  PN_REQUIRE(batch > 0 && T > 0 && T <= 16 && pixels > 0 && heads > 0, "pn_attention_temporal_f32: bad geometry (T <= 16)");
-  PN_REQUIRE(ld % 4 == 0 && ld >= (int64_t)heads * head_dim, "pn_attention_temporal_f32: bad token stride");
-  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_attention_temporal_f32: operand_mode %d", operand_mode);
+int attention_temporal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t T, int64_t pixels,
+                           int32_t heads, int32_t head_dim, int64_t ld, int64_t out_ld, float scale, int operand_mode,
+                           void* stream_v) {
+  PN_REQUIRE(q && k && v && out, "pn_attention_temporal: null pointer");
+  PN_REQUIRE(head_dim == 64 || head_dim == 80, "pn_attention_temporal: head_dim %d unsupported (64 or 80)", head_dim);
+  PN_REQUIRE(batch > 0 && T > 0 && T <= 16 && pixels > 0 && heads > 0, "pn_attention_temporal: bad geometry (T <= 16)");
+  PN_REQUIRE(ld % 4 == 0 && ld >= (int64_t)heads * head_dim, "pn_attention_temporal: bad token stride");
+  PN_REQUIRE(out_ld == (int64_t)heads * head_dim, "pn_attention_temporal: out_ld must equal heads*head_dim (dense operand)");
   const long long total = batch * T * pixels * heads;
   const long long blocks = (total + 127) / 128;
-  PN_REQUIRE(blocks < (1ll << 31), "pn_attention_temporal_f32: grid too large");
+  PN_REQUIRE(blocks < (1ll << 31), "pn_attention_temporal: grid too large");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   const float sl2 = scale * 1.4426950408889634f;
   if (head_dim == 64)
@@ -311,3 +307,5 @@ extern "C" int pn_attention_temporal_f32(const float* q, const float* k, const f
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
+
+}  // namespace pn

@@ -1,6 +1,6 @@
 // Cross-frame (temporal) self-attention: every pixel attends over its T <= 16 frames (attention.py:1116-1125 feeding
-// CrossAttention.forward :229-291 with context=None). Sequences this short cannot fill a 128-row UMMA tile (tcgen05 needs
-// M >= 64 rows of ONE problem), so each warp runs one (sequence b, pixel p, head) problem on the warp-level tensor path:
+// CrossAttention.forward :229-291 with context=None). Sequences this short cannot fill a 64-row wgmma tile (wgmma needs
+// M = 64 rows of ONE problem), so each warp runs one (sequence b, pixel p, head) problem on the warp-level tensor path:
 // S = Q K^T as m16n8k16 bf16 MMAs (4 per 8 keys), fp32 softmax on the accumulator fragment, O = P V as 8 more MMAs with
 // the S fragment re-used as the A operand. The op is HBM-bound (reads q,k,v once, writes o once); the scalar version of
 // this kernel spent ~800 instructions per problem and ran at a third of that roofline.
@@ -269,7 +269,13 @@ __global__ void __launch_bounds__((CA_MAXL / 16) * 32) attn_causal_kernel(const 
 using namespace pn;
 
 extern "C" int pn_attention_causal(const void* q, const void* k, const void* v, void* out, int64_t batch, int64_t L,
-                                   int32_t heads, int32_t head_dim, int64_t ld, int64_t out_ld, float scale, void* stream_v) {
+                                   int32_t heads, int32_t head_dim, int64_t ld, int64_t out_ld, float scale, int operand_mode,
+                                   void* stream_v) {
+  if (operand_mode == PN_OPERAND_SPLIT3 || operand_mode == PN_OPERAND_F32)
+    return attention_causal_f32(reinterpret_cast<const float*>(q), reinterpret_cast<const float*>(k),
+                                reinterpret_cast<const float*>(v), out, batch, L, heads, head_dim, ld, out_ld, scale, operand_mode,
+                                stream_v);
+  PN_REQUIRE(operand_mode == PN_OPERAND_BF16, "pn_attention_causal: operand_mode %d unsupported (0, 1 or 2)", operand_mode);
   PN_REQUIRE(q && k && v && out, "pn_attention_causal: null pointer");
   PN_REQUIRE(head_dim == CA_D, "pn_attention_causal: head_dim %d unsupported (64)", head_dim);
   PN_REQUIRE(L >= 1 && L <= CA_MAXL, "pn_attention_causal: L=%lld out of range 1..128", (long long)L);
@@ -293,7 +299,12 @@ extern "C" int pn_attention_causal(const void* q, const void* k, const void* v, 
 
 extern "C" int pn_attention_temporal(const void* q, const void* k, const void* v, void* out, int64_t batch, int64_t T,
                                      int64_t pixels, int32_t heads, int32_t head_dim, int64_t ld, int64_t out_ld,
-                                     float scale, void* stream_v) {
+                                     float scale, int operand_mode, void* stream_v) {
+  if (operand_mode == PN_OPERAND_SPLIT3 || operand_mode == PN_OPERAND_F32)
+    return attention_temporal_f32(reinterpret_cast<const float*>(q), reinterpret_cast<const float*>(k),
+                                  reinterpret_cast<const float*>(v), out, batch, T, pixels, heads, head_dim, ld, out_ld, scale,
+                                  operand_mode, stream_v);
+  PN_REQUIRE(operand_mode == PN_OPERAND_BF16, "pn_attention_temporal: operand_mode %d unsupported (0, 1 or 2)", operand_mode);
   PN_REQUIRE(q && k && v && out, "pn_attention_temporal: null pointer");
   PN_REQUIRE(head_dim == 64 || head_dim == 80, "pn_attention_temporal: head_dim %d unsupported (64 or 80)", head_dim);
   PN_REQUIRE(T >= 1 && T <= TA_MAXT, "pn_attention_temporal: T=%lld out of range 1..16", (long long)T);

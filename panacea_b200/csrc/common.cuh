@@ -8,6 +8,8 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+struct pn_attn_args;      // include/panacea_b200.h
+
 namespace pn {
 
 // Error codes returned over the C ABI (see include/panacea_b200.h).
@@ -46,5 +48,14 @@ int stride_grid(size_t total, int threads = 256);
 // opt in to `bytes` of dynamic shared memory for `func` on the current device (once per device and size);
 // `max_carveout` also asks for the largest shared-memory carveout, for kernels that plan on several CTAs per SM
 int ensure_dyn_smem(const void* func, size_t bytes, bool max_carveout = false);
+
+// Parity-mode attention (attn_f32.cu): fp32 q/k/v, fp32 math on CUDA cores, the output written as the operand of the
+// to_out GEMM in operand_mode. pn_attention / pn_attention_temporal / pn_attention_causal call these for the fp32 modes.
+int attention_f32(const pn_attn_args* a, int operand_mode, void* stream);
+int attention_temporal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t T, int64_t pixels,
+                           int32_t heads, int32_t head_dim, int64_t ld, int64_t out_ld, float scale, int operand_mode,
+                           void* stream);
+int attention_causal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t L, int32_t heads,
+                         int32_t head_dim, int64_t ld, int64_t out_ld, float scale, int operand_mode, void* stream);
 
 }  // namespace pn

@@ -1,4 +1,4 @@
-// Direct 3x3 convolution on CUDA cores for the layers whose channel counts cannot feed a 64-wide UMMA K block:
+// Direct 3x3 convolution on CUDA cores for the layers whose channel counts cannot feed a 64-wide wgmma K block:
 // the UNet/ControlNet stems (8 -> 320, openaimodel.py:977), the output head (320 -> 4, openaimodel.py:1251) and the
 // BEV hint stem (19 -> 16 -> 16 -> 32 -> 32 -> 96 -> 96 -> 256 -> 320 with strides 1,1,2,1,2,1,2,1,
 // controlmodel.py:43-59). The hint stem is step-invariant and runs once per sample; stem and head are <0.02 % of

@@ -2,7 +2,7 @@
 //
 //  PN_OP_BF16   : bf16 [rows, C]                     (the fast path: bf16 products, fp32 accumulation)
 //  PN_OP_SPLIT3 : bf16 [rows, 3C] = [hi | lo | hi]   (parity mode) with hi = bf16(v), lo = bf16(v - hi).
-//                 Against weights packed as [W_hi | W_hi | W_lo] per tap the SAME tcgen05 GEMM kernel computes
+//                 Against weights packed as [W_hi | W_hi | W_lo] per tap the SAME wgmma GEMM kernel computes
 //                 hi*W_hi + lo*W_hi + hi*W_lo = v*W up to the dropped lo*W_lo term (2^-18 relative): fp32-class
 //                 products on the bf16 tensor pipe by K-concatenation, no kernel change.
 //  PN_OP_F32    : fp32 [rows, C]                     (consumers that are CUDA-core kernels in parity mode)

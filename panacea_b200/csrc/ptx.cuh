@@ -34,7 +34,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// generic-proxy writes -> visible to the async proxy (TMA store / UMMA reads of smem)
+// generic-proxy writes -> visible to the async proxy (TMA store / wgmma reads of smem)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }

@@ -294,57 +294,45 @@ class Engine:
         return ops.gemm(tn2, W[k + ".outt.w"], bias=W[k + ".outt.b"], taps=(3, 1), residual=h2, residual2=x, out=h2).view(Fr, H, Wd, C)
 
     def _transformer(self, W, t: str, y, heads, mode, geom, kv):
-        """BasicTransformerBlock._forward (attention.py:726-747) on the fp32 token stream y [tokens, C]."""
-        ops = self.ops
-        dt = ops.qkv_dtype
+        """BasicTransformerBlock._forward (attention.py:726-747) on the token stream y [tokens, C] (ops.token_dtype).
+
+        A folded block (W[t + ".fold"]) takes y = (stream, its row statistics from proj_in) and folds norm1 and norm2 into
+        the GEMMs around the bf16 token stream: every GEMM that writes the stream also emits the per-row (sum, sum of
+        squares) of what it stored, and the GEMM that consumes LN(stream) multiplies the un-normalised stream by
+        W diag(gamma) and finishes the normalisation in its epilogue. No LayerNorm kernel, no normalised copy of the
+        stream. norm3 stays a kernel: the GEGLU epilogue is the long pole of ff1 at level 0, a rank-1 correction there
+        would lengthen it."""
+        ops, dt = self.ops, self.ops.qkv_dtype
         Fr, H, Wd, C, b, T = geom
-        if W[t + ".fold"]:
-            return self._transformer_folded(W, t, y, heads, mode, geom, kv)
-        n1 = ops.layernorm(y, W[t + ".norm1.g"], W[t + ".norm1.b"])
-        qkv = ops.gemm(n1, W[t + ".qkv.w"], out_dtype=dt)
+        fold = W[t + ".fold"]
+        y, st = y if fold else (y, None)
+        stats_out = {"ln_stats_out": True} if fold else {}
+
+        def ln_gemm(stream, stats, norm, proj):
+            """LN_norm(stream) W_proj^T: folded into the GEMM, or a LayerNorm kernel and then the GEMM"""
+            if fold:
+                return ops.gemm(stream, W[f"{t}.{proj}.w"], bias=W[f"{t}.{proj}.t"], out_dtype=dt, ln=(stats, W[f"{t}.{proj}.s"], 1e-5))
+            return ops.gemm(ops.layernorm(stream, W[f"{t}.{norm}.g"], W[f"{t}.{norm}.b"]), W[f"{t}.{proj}.w"], out_dtype=dt)
+
+        qkv = ln_gemm(y, st, "norm1", "qkv")
         if mode == "temporal":
             o = ops.attention_temporal(qkv.view(b, T, H * Wd, 3 * C), heads)
         else:
             V = self.cfg.num_views
             o = ops.attention_view(qkv.view(Fr, H, V, Wd // V, 3 * C), heads, mode == "cross", CROSS_VIEW_NEIGHBOURS)
-        tok = y.dtype                                    # token stream: bf16 in the fast path (ops.token_dtype), fp32 otherwise
-        y = ops.gemm(o.view(-1, o.shape[-1]), W[t + ".attn1.o.w"], bias=W[t + ".attn1.o.b"], residual=y, out=y, out_dtype=tok)
-        n2 = ops.layernorm(y, W[t + ".norm2.g"], W[t + ".norm2.b"])
-        q = ops.gemm(n2, W[t + ".q2.w"], out_dtype=dt)
+        r = ops.gemm(o.view(-1, o.shape[-1]), W[t + ".attn1.o.w"], bias=W[t + ".attn1.o.b"], residual=y, out=y, out_dtype=y.dtype,
+                     **stats_out)
+        y, st = r if fold else (r, None)
+        q = ln_gemm(y, st, "norm2", "q2")
         o = ops.attention_text(q.view(b, T * H * Wd, C), kv, heads)
-        y = ops.gemm(o.view(-1, o.shape[-1]), W[t + ".attn2.o.w"], bias=W[t + ".attn2.o.b"], residual=y, out=y, out_dtype=tok)
+        y = ops.gemm(o.view(-1, o.shape[-1]), W[t + ".attn2.o.w"], bias=W[t + ".attn2.o.b"], residual=y, out=y, out_dtype=y.dtype)
         n3 = ops.layernorm(y, W[t + ".norm3.g"], W[t + ".norm3.b"])
         ff = ops.gemm(n3, W[t + ".ff1.w"], bias=W[t + ".ff1.b"], geglu=True, out_dtype=ops.act_dtype)
         # the block's output is only ever consumed as the bf16 operand of proj_out: emit it in that form directly
         # (saves the fp32 write, the cast kernel's fp32 read and one launch per transformer block)
-        if ops.fused_operand_emit:
+        if fold or ops.fused_operand_emit:
             return ops.gemm(ff, W[t + ".ff2.w"], bias=W[t + ".ff2.b"], residual=y, out_dtype=torch.bfloat16)
-        return ops.gemm(ff, W[t + ".ff2.w"], bias=W[t + ".ff2.b"], residual=y, out=y, out_dtype=tok)
-
-    def _transformer_folded(self, W, t: str, ys, heads, mode, geom, kv):
-        """The same block with the three LayerNorms folded into the GEMMs around the bf16 token stream: every GEMM that
-        writes the stream also emits the per-row (sum, sum of squares) of what it stored, and the GEMM that consumes
-        LN(stream) multiplies the un-normalised stream by W diag(gamma) and finishes the normalisation in its epilogue.
-        No LayerNorm kernel, no normalised copy of the stream."""
-        ops, dt = self.ops, self.ops.qkv_dtype
-        Fr, H, Wd, C, b, T = geom
-        y, st = ys                                       # stream + row statistics from proj_in
-        eps = 1e-5
-        qkv = ops.gemm(y, W[t + ".qkv.w"], bias=W[t + ".qkv.t"], out_dtype=dt, ln=(st, W[t + ".qkv.s"], eps))
-        if mode == "temporal":
-            o = ops.attention_temporal(qkv.view(b, T, H * Wd, 3 * C), heads)
-        else:
-            V = self.cfg.num_views
-            o = ops.attention_view(qkv.view(Fr, H, V, Wd // V, 3 * C), heads, mode == "cross", CROSS_VIEW_NEIGHBOURS)
-        y, st = ops.gemm(o.view(-1, C), W[t + ".attn1.o.w"], bias=W[t + ".attn1.o.b"], residual=y, out=y, out_dtype=y.dtype, ln_stats_out=True)
-        q = ops.gemm(y, W[t + ".q2.w"], bias=W[t + ".q2.t"], out_dtype=dt, ln=(st, W[t + ".q2.s"], eps))
-        o = ops.attention_text(q.view(b, T * H * Wd, C), kv, heads)
-        # norm3 stays a kernel: the GEGLU epilogue is the long pole of ff1 at level 0, a rank-1 correction there would
-        # lengthen it
-        y = ops.gemm(o.view(-1, C), W[t + ".attn2.o.w"], bias=W[t + ".attn2.o.b"], residual=y, out=y, out_dtype=y.dtype)
-        n3 = ops.layernorm(y, W[t + ".norm3.g"], W[t + ".norm3.b"])
-        ff = ops.gemm(n3, W[t + ".ff1.w"], bias=W[t + ".ff1.b"], geglu=True, out_dtype=ops.act_dtype)
-        return ops.gemm(ff, W[t + ".ff2.w"], bias=W[t + ".ff2.b"], residual=y, out_dtype=torch.bfloat16)
+        return ops.gemm(ff, W[t + ".ff2.w"], bias=W[t + ".ff2.b"], residual=y, out=y, out_dtype=y.dtype)
 
     def _stt(self, W, st: Stage, x):
         """SpatialTemporalTransformer.forward (attention.py:1064-1134): intra-view, cross-view, temporal."""

@@ -55,7 +55,7 @@ def split3(t: torch.Tensor, taps: int = 1) -> torch.Tensor:
 
 
 def _attn_args(q, k, v, out, *, q_ld, kv_ld, F, H, V, W, Hk, Vk, Wk, heads, head_dim, views):
-    """pn_attn_args for pn_attention / pn_attention_f32: q, k, v, out are device addresses, the output dense
+    """pn_attn_args for pn_attention: q, k, v, out are device addresses, the output dense
     ([tokens, heads * head_dim]); query view v attends the key views views[v]."""
     a = _lib.AttnArgs()
     a.q, a.k, a.v, a.out = q, k, v, out
@@ -244,63 +244,68 @@ class NativeOps:
         return y
 
     # ------------------------------------------------------------------ attention
+    # Inputs are qkv_dtype (bf16, or fp32 in parity mode, which runs attention in fp32 on CUDA cores); outputs are the
+    # operand of the to_out GEMM in this op set's operand_mode.
     def _attention(self, q, k, v, out, **geometry):
-        _lib.check(self.lib.pn_attention(C.byref(_attn_args(q, k, v, out, **geometry)), _stream()), "pn_attention")
+        _lib.check(self.lib.pn_attention(C.byref(_attn_args(q, k, v, out, **geometry)), self.operand_mode, _stream()), "pn_attention")
         self.launches += 1
 
+    def _qkv_ok(self, *ts):
+        return all(t.is_cuda and t.dtype == self.qkv_dtype and t.is_contiguous() for t in ts)
+
     def attention_view(self, qkv, heads, cross, neighbours):
-        """qkv bf16 [F, H, V, w, 3C] (fused q|k|v channels) -> bf16 [F, H, V, w, C].
+        """qkv [F, H, V, w, 3C] (fused q|k|v channels) -> operand [F, H, V, w, C].
         cross=False: each view attends itself; cross=True: view v attends neighbours[v]."""
-        _req(qkv.is_cuda and qkv.dtype == BF16 and qkv.is_contiguous() and qkv.dim() == 5, "attention_view: qkv bf16 [F,H,V,w,3C]")
+        _req(self._qkv_ok(qkv) and qkv.dim() == 5, f"attention_view: qkv {self.qkv_dtype} [F,H,V,w,3C]")
         Fr, H, V, w, C3 = qkv.shape
         Cc = C3 // 3
         d = Cc // heads
         _req(Cc == heads * d and d in (64, 80), "attention_view: head_dim must be 64 or 80")
-        out = torch.empty((Fr, H, V, w, Cc), device=qkv.device, dtype=BF16)
+        out = self._operand_empty((Fr, H, V, w, Cc), qkv.device)
         views = [list(neighbours[v]) for v in range(V)] if cross else [[v] for v in range(V)]
-        base = qkv.data_ptr()
-        self._attention(base, base + 2 * Cc, base + 4 * Cc, out.data_ptr(), q_ld=C3, kv_ld=C3, F=Fr, H=H, V=V, W=w, Hk=H, Vk=V, Wk=w,
+        base, row = qkv.data_ptr(), Cc * qkv.element_size()
+        self._attention(base, base + row, base + 2 * row, out.data_ptr(), q_ld=C3, kv_ld=C3, F=Fr, H=H, V=V, W=w, Hk=H, Vk=V, Wk=w,
                         heads=heads, head_dim=d, views=views)
         return out
 
     def attention_text(self, q, kv, heads):
-        """q bf16 [b, Nq, C]; kv bf16 [b, Nk, 2C] (k | v channels), Nk <= 128 -> bf16 [b, Nq, C]."""
-        _req(q.is_cuda and q.dtype == BF16 and q.is_contiguous() and kv.dtype == BF16 and kv.is_contiguous(), "attention_text: bf16 contiguous")
+        """q [b, Nq, C]; kv [b, Nk, 2C] (k | v channels) -> operand [b, Nq, C]. bf16 mode: Nk <= 128 (head_dim 64) / 112 (80)."""
+        _req(self._qkv_ok(q, kv), f"attention_text: {self.qkv_dtype} contiguous")
         b, Nq, Cc = q.shape
         Nk = kv.shape[1]
         d = Cc // heads
-        _req(kv.shape[0] == b and kv.shape[2] == 2 * Cc and Cc == heads * d and d in (64, 80) and Nk <= (128 if d == 64 else 112),
-             "attention_text: bad shapes")
-        out = torch.empty_like(q)
+        _req(kv.shape[0] == b and kv.shape[2] == 2 * Cc and Cc == heads * d and d in (64, 80)
+             and (self.operand_mode != OP_BF16 or Nk <= (128 if d == 64 else 112)), "attention_text: bad shapes")
+        out = self._operand_empty((b, Nq, Cc), q.device)
         base = kv.data_ptr()
-        self._attention(q.data_ptr(), base, base + 2 * Cc, out.data_ptr(), q_ld=Cc, kv_ld=2 * Cc, F=b, H=1, V=1, W=Nq, Hk=1, Vk=1,
-                        Wk=Nk, heads=heads, head_dim=d, views=[[0]])
+        self._attention(q.data_ptr(), base, base + Cc * kv.element_size(), out.data_ptr(), q_ld=Cc, kv_ld=2 * Cc, F=b, H=1, V=1,
+                        W=Nq, Hk=1, Vk=1, Wk=Nk, heads=heads, head_dim=d, views=[[0]])
         return out
 
     def attention_temporal(self, qkv, heads):
-        """qkv bf16 [b, T, P, 3C] -> bf16 [b, T, P, C]; softmax over the T frames of each pixel."""
-        _req(qkv.is_cuda and qkv.dtype == BF16 and qkv.is_contiguous() and qkv.dim() == 4, "attention_temporal: qkv bf16 [b,T,P,3C]")
+        """qkv [b, T, P, 3C] -> operand [b, T, P, C]; softmax over the T frames of each pixel."""
+        _req(self._qkv_ok(qkv) and qkv.dim() == 4, f"attention_temporal: qkv {self.qkv_dtype} [b,T,P,3C]")
         b, T, P, C3 = qkv.shape
         Cc = C3 // 3
         d = Cc // heads
         _req(Cc == heads * d and d in (64, 80), "attention_temporal: head_dim must be 64 or 80")
-        out = torch.empty((b, T, P, Cc), device=qkv.device, dtype=BF16)
-        base = qkv.data_ptr()
-        _lib.check(self.lib.pn_attention_temporal(base, base + 2 * Cc, base + 4 * Cc, out.data_ptr(), b, T, P, heads, d, C3, Cc,
-                                                 d ** -0.5, _stream()), "pn_attention_temporal")
+        out = self._operand_empty((b, T, P, Cc), qkv.device)
+        base, row = qkv.data_ptr(), Cc * qkv.element_size()
+        _lib.check(self.lib.pn_attention_temporal(base, base + row, base + 2 * row, out.data_ptr(), b, T, P, heads, d, C3, Cc,
+                                                 d ** -0.5, self.operand_mode, _stream()), "pn_attention_temporal")
         self.launches += 1
         return out
 
     def attention_causal(self, qkv, heads):
-        """qkv bf16 [b, L, 3C] (fused q|k|v channels, L <= 128) -> bf16 [b, L, C]; token i attends keys j <= i."""
-        _req(qkv.is_cuda and qkv.dtype == BF16 and qkv.is_contiguous() and qkv.dim() == 3, "attention_causal: qkv bf16 [b,L,3C]")
+        """qkv [b, L, 3C] (fused q|k|v channels, L <= 128) -> operand [b, L, C]; token i attends keys j <= i."""
+        _req(self._qkv_ok(qkv) and qkv.dim() == 3, f"attention_causal: qkv {self.qkv_dtype} [b,L,3C]")
         b, L, C3 = qkv.shape
         Cc = C3 // 3
         _req(Cc == heads * 64 and 1 <= L <= 128, "attention_causal: needs head_dim 64 and L <= 128")
-        out = torch.empty((b, L, Cc), device=qkv.device, dtype=BF16)
-        base = qkv.data_ptr()
-        _lib.check(self.lib.pn_attention_causal(base, base + 2 * Cc, base + 4 * Cc, out.data_ptr(), b, L, heads, 64, C3, Cc,
-                                               64 ** -0.5, _stream()), "pn_attention_causal")
+        out = self._operand_empty((b, L, Cc), qkv.device)
+        base, row = qkv.data_ptr(), Cc * qkv.element_size()
+        _lib.check(self.lib.pn_attention_causal(base, base + row, base + 2 * row, out.data_ptr(), b, L, heads, 64, C3, Cc,
+                                               64 ** -0.5, self.operand_mode, _stream()), "pn_attention_causal")
         self.launches += 1
         return out
 
@@ -508,8 +513,8 @@ class ParityOps(NativeOps):
     """fp32-class precision mode (the literal rtol 1e-3 / atol 1e-4 bar of BASELINE.json against the reference's fp32
     math). Same kernels, different operand encoding: every producer stores the GEMM operand as bf16 [hi | lo | hi]
     (3C wide), weights are packed [W_hi | W_hi | W_lo], so the wgmma GEMM/conv kernel computes fp32-class products by
-    K-concatenation; attention runs in fp32 on CUDA cores (pn_attention_f32); GEGLU uses the exact erf; the
-    time-embedding linears read fp32 weights. About 3-4x the cost of the bf16 path."""
+    K-concatenation; attention runs in fp32 on CUDA cores; GEGLU uses the exact erf; the time-embedding linears read
+    fp32 weights. About 3-4x the cost of the bf16 path."""
 
     operand_mode = OP_SPLIT3
     operand_mult = 3
@@ -538,56 +543,3 @@ class ParityOps(NativeOps):
             return y
         _req(out_dtype == F32, "parity gemm: outputs are fp32 (operands are produced by cast_operand)")
         return super().gemm(a, w, out_dtype=F32, **kw)
-
-    # ------------------------------------------------------------------ attention (fp32, CUDA cores)
-    def _attention_f32(self, q, k, v, out, **geometry):
-        _lib.check(self.lib.pn_attention_f32(C.byref(_attn_args(q, k, v, out, **geometry)), self.operand_mode, _stream()),
-                   "pn_attention_f32")
-        self.launches += 1
-
-    def attention_view(self, qkv, heads, cross, neighbours):
-        _req(qkv.is_cuda and qkv.dtype == F32 and qkv.is_contiguous() and qkv.dim() == 5, "attention_view(parity): qkv fp32 [F,H,V,w,3C]")
-        Fr, H, V, w, C3 = qkv.shape
-        Cc = C3 // 3
-        d = Cc // heads
-        out = self._operand_empty((Fr, H, V, w, Cc), qkv.device)
-        views = [list(neighbours[v]) for v in range(V)] if cross else [[v] for v in range(V)]
-        base = qkv.data_ptr()
-        self._attention_f32(base, base + 4 * Cc, base + 8 * Cc, out.data_ptr(), q_ld=C3, kv_ld=C3, F=Fr, H=H, V=V, W=w, Hk=H, Vk=V, Wk=w,
-                            heads=heads, head_dim=d, views=views)
-        return out
-
-    def attention_text(self, q, kv, heads):
-        _req(q.is_cuda and q.dtype == F32 and q.is_contiguous() and kv.dtype == F32 and kv.is_contiguous(), "attention_text(parity): fp32")
-        b, Nq, Cc = q.shape
-        Nk = kv.shape[1]
-        _req(kv.shape[0] == b and kv.shape[2] == 2 * Cc, "attention_text: bad shapes")
-        out = self._operand_empty((b, Nq, Cc), q.device)
-        base = kv.data_ptr()
-        self._attention_f32(q.data_ptr(), base, base + 4 * Cc, out.data_ptr(), q_ld=Cc, kv_ld=2 * Cc, F=b, H=1, V=1, W=Nq, Hk=1, Vk=1,
-                            Wk=Nk, heads=heads, head_dim=Cc // heads, views=[[0]])
-        return out
-
-    def attention_temporal(self, qkv, heads):
-        _req(qkv.is_cuda and qkv.dtype == F32 and qkv.is_contiguous() and qkv.dim() == 4, "attention_temporal(parity): qkv fp32 [b,T,P,3C]")
-        b, T, P, C3 = qkv.shape
-        Cc = C3 // 3
-        d = Cc // heads
-        out = self._operand_empty((b, T, P, Cc), qkv.device)
-        base = qkv.data_ptr()
-        _lib.check(self.lib.pn_attention_temporal_f32(base, base + 4 * Cc, base + 8 * Cc, out.data_ptr(), b, T, P, heads, d, C3, d ** -0.5,
-                                                     self.operand_mode, _stream()), "pn_attention_temporal_f32")
-        self.launches += 1
-        return out
-
-    def attention_causal(self, qkv, heads):
-        _req(qkv.is_cuda and qkv.dtype == F32 and qkv.is_contiguous() and qkv.dim() == 3, "attention_causal(parity): qkv fp32 [b,L,3C]")
-        b, L, C3 = qkv.shape
-        Cc = C3 // 3
-        _req(Cc == heads * 64 and 1 <= L <= 128, "attention_causal: needs head_dim 64 and L <= 128")
-        out = self._operand_empty((b, L, Cc), qkv.device)
-        base = qkv.data_ptr()
-        _lib.check(self.lib.pn_attention_causal_f32(base, base + 4 * Cc, base + 8 * Cc, out.data_ptr(), b, L, heads, 64, C3, 64 ** -0.5,
-                                                   self.operand_mode, _stream()), "pn_attention_causal_f32")
-        self.launches += 1
-        return out

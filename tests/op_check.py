@@ -27,7 +27,6 @@ from pathlib import Path
 import numpy as np
 import torch
 
-from clip_ref_ops import TextRefOps
 from torch_ref_ops import TorchRefOps64
 
 F32, BF16, F64 = torch.float32, torch.bfloat16, torch.float64
@@ -54,10 +53,6 @@ OP_CLASS = {"gemm": "gemm", "linear_small": "gemm", "groupnorm": "norm", "groupn
 
 class OpCheckError(AssertionError):
     pass
-
-
-class Ref64(TextRefOps, TorchRefOps64):
-    """fp64, pre-store reference of every op (the text-encoder ops included)."""
 
 
 # ------------------------------------------------------------------------------------------------ stored formats
@@ -126,7 +121,7 @@ def _overlaps(a, b):
 # ------------------------------------------------------------------------------------------------ element bounds
 def _abs_gemm(a, w, taps):
     """sum_k |a_k| |w_k| of every output element (fp64)"""
-    return Ref64().gemm(a.abs(), w.abs(), taps=taps)
+    return TorchRefOps64().gemm(a.abs(), w.abs(), taps=taps)
 
 
 def _norm_bound(ref, xhat, ratio, gamma, silu, fmt):
@@ -142,7 +137,7 @@ def _norm_bound(ref, xhat, ratio, gamma, silu, fmt):
 class _Checks:
     """fp64 reference and element bound of one call: each method returns (ref, bound, extra) on the snapshot."""
 
-    R = Ref64()
+    R = TorchRefOps64()
 
     # ---------------------------------------------------------------- gemm
     def gemm(self, got, a, w, *, bias=None, rowvec=None, rows_per_group=0, n_groups=0, residual=None, residual2=None,
@@ -329,7 +324,7 @@ class _Checks:
 # ------------------------------------------------------------------------------------------------ bitwise ops
 def _bitwise_ref(name, got, args, kw, weight_form=False):
     """the exact output of a layout / cast / embedding op, in the output's stored form"""
-    R = Ref64()
+    R = TorchRefOps64()
     if name == "token_embedding":
         return R.token_embedding(*args).float()
     if name == "concat_add":

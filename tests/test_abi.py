@@ -19,7 +19,7 @@ def test_header_declares_entry_points():
     assert "pn_gemm" in names and "pn_attention" in names and len(names) >= 20
 
 
-def test_library_exports_every_declared_symbol_of_abi_3():
+def test_library_exports_every_declared_symbol_of_abi_4():
     from panacea_b200 import _lib, build
     build.build()
     lib = _lib.load()
@@ -28,7 +28,7 @@ def test_library_exports_every_declared_symbol_of_abi_3():
         assert hasattr(lib, n), f"{n} declared in the header but not exported"
         assert n in _lib.SIGNATURES, f"{n} has no ctypes signature"
     assert set(_lib.SIGNATURES) == set(names)
-    assert lib.pn_abi_version() == 3
+    assert lib.pn_abi_version() == 4
 
 
 def test_struct_layout_matches_header_field_order():

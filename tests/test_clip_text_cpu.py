@@ -112,14 +112,14 @@ def test_real_vocabulary_matches_open_clip():
 
 # ------------------------------------------------------------------ engine orchestration
 def test_engine_orchestration_matches_the_reference_on_cpu():
-    from clip_ref_ops import TextRefOps
+    from torch_ref_ops import TorchRefOps
     from panacea_b200.text_encoder import TextEncoderEngine, text_param_spec
     g = torch.load(GOLDEN / "clip_text.pt")["small"]
     c = g["config"]
     P = clip_text_weights(c["vocab"], c["width"], c["layers"], c["seed"])
     spec = text_param_spec(c["vocab"], g["ctx"], c["width"], c["layers"])
     assert sorted(spec) == sorted(set(g["keys"]) - {"text_projection", "logit_scale"})
-    eng = TextEncoderEngine(TextRefOps())
+    eng = TextEncoderEngine(TorchRefOps())
     eng.pack(P)
     assert eng.heads == c["heads"]
     out = eng.encode(g["tokens"], g["layer_idx"])
@@ -128,9 +128,9 @@ def test_engine_orchestration_matches_the_reference_on_cpu():
 
 
 def test_engine_rejects_bad_head_dim_and_out_of_range_tokens():
-    from clip_ref_ops import TextRefOps
+    from torch_ref_ops import TorchRefOps
     from panacea_b200.text_encoder import TextEncoderEngine
-    eng = TextEncoderEngine(TextRefOps())
+    eng = TextEncoderEngine(TorchRefOps())
     with pytest.raises(NotImplementedError, match="head_dim"):
         eng.pack(clip_text_weights(50, 96, 1, 0))
     eng.pack(clip_text_weights(50, 64, 2, 0))

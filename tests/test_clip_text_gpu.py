@@ -1,4 +1,4 @@
-"""OpenCLIP text encoder on the GPU: the new kernels (pn_attention_causal and its fp32 twin, pn_gelu_operand,
+"""OpenCLIP text encoder on the GPU: the new kernels (pn_attention_causal in bf16 and fp32, pn_gelu_operand,
 pn_token_embedding) against torch, the whole tower in both precision modes against the UNMODIFIED reference
 (tests/golden/clip_text.pt), and the embedder inside the inference engine on tests/configs/tiny_inference.yaml."""
 import time

@@ -5,35 +5,17 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from clip_ref_ops import TextRefOps, TextSplitOps
 from oracle import cases as Cs
 from op_check import CHECKED, EXCLUDED, OpCheckError, checked
 from panacea_b200 import engine as E
 from panacea_b200 import netplan as NP
-from torch_ref_ops import TorchFoldOps, TorchRefOps, TorchRefOps64, TorchSplitOps, _enc
+from torch_ref_ops import TorchFoldOps, TorchRefOps, TorchRefOps64, TorchSplitOps
 
 
 def _split(sd):
     up = {k[len("diffusion_model."):]: v for k, v in sd.items() if not k.startswith("diffusion_model.controlnet.")}
     cp = {k[len("diffusion_model.controlnet."):]: v for k, v in sd.items() if k.startswith("diffusion_model.controlnet.")}
     return up, cp
-
-
-class FoldOps(TorchFoldOps, TextRefOps):
-    pass
-
-
-class TextOps(TextRefOps):
-    """torch's fp32 CPU erf errs by several ulp near erf = -1; the kernel's erff by <= 2 ulp: emulate that with a
-    correctly rounded GELU"""
-
-    def gelu_operand(self, x):
-        return F.gelu(x.double()).float()
-
-
-class TextSplitOps2(TextSplitOps):
-    def gelu_operand(self, x):
-        return _enc(F.gelu(x.double()).float())
 
 
 def _eps_run(ops, name="tiny_3to1"):
@@ -66,7 +48,7 @@ def test_every_public_op_is_checked_or_excluded():
 
 
 def test_an_op_without_a_checker_is_refused():
-    class WithNewKernel(FoldOps):
+    class WithNewKernel(TorchFoldOps):
         def new_kernel(self, x):
             return x
     ops = checked(WithNewKernel)()
@@ -88,7 +70,7 @@ def test_fp64_reference_matches_fp32_reference():
 
 
 @pytest.mark.parametrize("name", ["tiny_3to1", "small_hd64"])
-@pytest.mark.parametrize("base", [FoldOps, TorchSplitOps], ids=["fold", "split"])
+@pytest.mark.parametrize("base", [TorchFoldOps, TorchSplitOps], ids=["fold", "split"])
 def test_clean_emulation_passes_every_call(name, base):
     ops = checked(base)()
     eps = _eps_run(ops, name)
@@ -105,15 +87,14 @@ def test_clean_vae_and_text_emulations_pass(parity):
     from oracle.make_golden import VAE_DDCONFIG, vae_decoder_input, vae_decoder_weights, vae_encoder_input
     from panacea_b200.text_encoder import TextEncoderEngine
     from panacea_b200.vae import VAEDecoderEngine, VAEEncoderEngine
-    from test_vae_parity_cpu import TorchSplitOpsVAE
-    base = TorchSplitOpsVAE if parity else TorchRefOps
+    base = TorchSplitOps if parity else TorchRefOps
     for Eng, run, inp in ((VAEDecoderEngine, "decode", vae_decoder_input()), (VAEEncoderEngine, "encode_moments", vae_encoder_input())):
         ops = checked(base)()
         eng = Eng(VAE_DDCONFIG, ops)
         eng.pack(vae_decoder_weights(eng.spec))
         assert torch.isfinite(getattr(eng, run)(inp)).all()
         assert "gemm" in ops.stats and "groupnorm" in ops.stats
-    ops = checked(TextSplitOps2 if parity else TextOps)()
+    ops = checked(base)()
     _text_run(ops)
     assert {"token_embedding", "layernorm", "attention_causal", "gelu_operand", "gemm"} <= set(ops.stats)
 
@@ -131,7 +112,7 @@ class _Once:
         return n[name] == self.at
 
 
-class SkipKBlock(_Once, FoldOps):
+class SkipKBlock(_Once, TorchFoldOps):
     def gemm(self, a, w, **kw):
         if self._fire("gemm", w.shape[1] >= 256):
             w = w.clone()
@@ -139,7 +120,7 @@ class SkipKBlock(_Once, FoldOps):
         return super().gemm(a, w, **kw)
 
 
-class ShiftedTap(_Once, FoldOps):
+class ShiftedTap(_Once, TorchFoldOps):
     def gemm(self, a, w, *, taps=(1, 1), **kw):
         if self._fire("gemm", taps == (3, 3)):
             C = a.shape[-1]
@@ -156,14 +137,14 @@ class ShiftedTap(_Once, FoldOps):
         return super().gemm(a, w, taps=taps, **kw)
 
 
-class RowvecOffByOne(_Once, FoldOps):
+class RowvecOffByOne(_Once, TorchFoldOps):
     def gemm(self, a, w, *, rowvec=None, rows_per_group=0, n_groups=0, **kw):
         if self._fire("gemm", rowvec is not None and not torch.equal(rowvec[0], rowvec[1])):
             rowvec = torch.roll(rowvec, 1, dims=0)   # group g gets the vector of group g - 1
         return super().gemm(a, w, rowvec=rowvec, rows_per_group=rows_per_group, n_groups=n_groups, **kw)
 
 
-class SwappedQueryRows(_Once, FoldOps):
+class SwappedQueryRows(_Once, TorchFoldOps):
     def attention_view(self, qkv, heads, cross, neighbours):
         out = super().attention_view(qkv, heads, cross, neighbours)
         if self._fire("attention_view", cross):
@@ -172,7 +153,7 @@ class SwappedQueryRows(_Once, FoldOps):
         return out
 
 
-class WideChannelWrite(_Once, FoldOps):
+class WideChannelWrite(_Once, TorchFoldOps):
     def nchw_to_nhwc(self, x, out=None, ch_off=0):
         r = super().nchw_to_nhwc(x, out=out, ch_off=ch_off)
         if self._fire("nchw_to_nhwc", out is not None and out.shape[-1] > ch_off + x.shape[1]):
@@ -180,7 +161,7 @@ class WideChannelWrite(_Once, FoldOps):
         return r
 
 
-class ModifiesInput(_Once, FoldOps):
+class ModifiesInput(_Once, TorchFoldOps):
     def groupnorm(self, x, *a, **k):
         r = super().groupnorm(x, *a, **k)
         if self._fire("groupnorm"):
@@ -192,7 +173,7 @@ class ModifiesInput(_Once, FoldOps):
     (SkipKBlock, "gemm", "engine.py"),
     (ShiftedTap, "gemm", "_run_block [input_blocks.0.0]"),
     (RowvecOffByOne, "gemm", "_stt"),
-    (SwappedQueryRows, "attention_view", "_transformer_folded"),
+    (SwappedQueryRows, "attention_view", "_transformer"),
     (WideChannelWrite, "nchw_to_nhwc", "prepare_hint"),
     (ModifiesInput, "groupnorm", "_res"),
 ], ids=["skip_k_block", "shifted_tap", "rowvec_off_by_one", "swapped_query_rows", "write_outside_channel_slice",

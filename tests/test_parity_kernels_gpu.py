@@ -106,6 +106,23 @@ def test_attention_text_and_temporal_f32(ops, d):
         assert _rel(o, r) < 1e-5
 
 
+def test_attention_entry_points_refuse_other_operand_modes(ops):
+    """each attention entry point serves bf16, split3 and fp32; any other operand_mode, the weight form included, is
+    refused with a message that names it"""
+    import ctypes
+    from panacea_b200.ops import OP_SPLIT3_B, _attn_args, _stream
+    qkv = torch.zeros(1, 8, 3 * 64, device="cuda")
+    out = torch.empty(1, 8, 3 * 64, device="cuda", dtype=torch.bfloat16)
+    p, o, lib = qkv.data_ptr(), out.data_ptr(), ops.lib
+    for mode in (OP_SPLIT3_B, 7):
+        a = _attn_args(p, p, p, o, q_ld=192, kv_ld=192, F=1, H=1, V=1, W=8, Hk=1, Vk=1, Wk=8, heads=1, head_dim=64, views=[[0]])
+        for call in (lambda: lib.pn_attention(ctypes.byref(a), mode, _stream()),
+                     lambda: lib.pn_attention_temporal(p, p, p, o, 1, 8, 1, 1, 64, 192, 64, 0.125, mode, _stream()),
+                     lambda: lib.pn_attention_causal(p, p, p, o, 1, 8, 1, 64, 192, 64, 0.125, mode, _stream())):
+            assert call() == -1 and f"operand_mode {mode}".encode() in lib.pn_last_error()
+    torch.cuda.synchronize()
+
+
 def test_geglu_pass_uses_the_exact_erf(ops):
     from panacea_b200.ops import geglu_pack, split3
     M, K, inner = 1000, 320, 1280

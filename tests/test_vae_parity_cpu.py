@@ -12,27 +12,9 @@ from oracle.make_golden import VAE_DDCONFIG, vae_decoder_input, vae_decoder_weig
 from panacea_b200.vae import VAEDecoderEngine, VAEEncoderEngine, decoder_param_spec, encoder_param_spec
 from test_eps_parity_gpu import BOUNDS
 from tools.make_vae_golden import FULL_WIDTH_DDCONFIG, full_width_inputs
-from torch_ref_ops import TorchSplitOps, _enc
+from torch_ref_ops import TorchSplitOps, _enc_weight_form
 
 GOLDEN = Path(__file__).resolve().parent / "golden"
-
-
-def _enc_weight_form(x):
-    """operand.cuh PN_OP_SPLIT3_B: fp32 [..., C] -> bf16 [..., 3C] = [hi | hi | lo], the layout split3() packs weights in."""
-    hi = x.to(torch.bfloat16)
-    lo = (x - hi.float()).to(torch.bfloat16)
-    return torch.cat([hi, hi, lo], dim=-1)
-
-
-class TorchSplitOpsVAE(TorchSplitOps):
-    """TorchSplitOps plus the two operand forms of the VAE's parity attention: the weight-form cast
-    (pn_cast_operand mode 3) and the split3 row softmax (pn_softmax_rows_operand mode 1)."""
-
-    def cast_operand(self, x, weight_form=False):
-        return _enc_weight_form(x) if weight_form else _enc(x)
-
-    def softmax_rows(self, s, scale):
-        return _enc(super().softmax_rows(s, scale))
 
 
 def _check_parity(name, got, ref):
@@ -60,7 +42,7 @@ def _cases():
 @pytest.mark.parametrize("case", ["small", "full_width"])
 def test_parity_decoder_orchestration_matches_the_reference(case):
     dd, g, dseed, _, z, _ = _cases()[case]
-    eng = VAEDecoderEngine(dd, TorchSplitOpsVAE())
+    eng = VAEDecoderEngine(dd, TorchSplitOps())
     eng.pack(vae_decoder_weights(eng.spec, seed=dseed))
     _check_parity(f"vae_decode_{case}", eng.decode(z), g["image"])
 
@@ -68,7 +50,7 @@ def test_parity_decoder_orchestration_matches_the_reference(case):
 @pytest.mark.parametrize("case", ["small", "full_width"])
 def test_parity_encoder_orchestration_matches_the_reference(case):
     dd, g, _, eseed, _, x = _cases()[case]
-    eng = VAEEncoderEngine(dd, TorchSplitOpsVAE())
+    eng = VAEEncoderEngine(dd, TorchSplitOps())
     eng.pack(vae_decoder_weights(eng.spec, seed=eseed))
     _check_parity(f"vae_encode_{case}", eng.encode_moments(x), g["moments"])
 
@@ -133,7 +115,7 @@ def test_engine_precision_reaches_the_first_stage():
 def test_frame_chunks_keep_every_groupnorm_split():
     """The planner allows a chunk size only where GroupNorm splits each frame the same way as one call over all frames
     (here a stand-in geometry: one frame per call doubles the split), and uses as few calls as possible."""
-    eng = VAEDecoderEngine(FULL_WIDTH_DDCONFIG, TorchSplitOpsVAE())
+    eng = VAEDecoderEngine(FULL_WIDTH_DDCONFIG, TorchSplitOps())
     eng.ops = type("Geometry", (), {"groupnorm_ctas_per_frame": staticmethod(lambda f, P, C: 132 // min(f, 2))})()
     assert eng.frame_chunks(8, (32, 384), 8) == [8]
     assert eng.frame_chunks(8, (32, 384), 2) == [2, 2, 2, 2]

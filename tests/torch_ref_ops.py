@@ -118,7 +118,7 @@ class TorchRefOps:
             y = F.silu(y)
         return y.reshape(b, P, C, T).permute(0, 3, 1, 2).contiguous()
 
-    def layernorm(self, x, gamma, beta, eps=1e-5):
+    def layernorm(self, x, gamma, beta, eps=1e-5, out_f32=False):
         return F.layer_norm(self._c(x), (x.shape[-1],), self._c(gamma), self._c(beta), eps)
 
     @staticmethod
@@ -155,6 +155,23 @@ class TorchRefOps:
         o = self._mha(seq(q), seq(k), seq(v), heads)
         return self._store(o.reshape(b, P, T, C).permute(0, 2, 1, 3).contiguous(), qkv.dtype)
 
+    def attention_causal(self, qkv, heads):
+        b, L, C3 = qkv.shape
+        C = C3 // 3
+        q, k, v = (t.reshape(b, L, heads, C // heads).transpose(1, 2) for t in self._c(qkv).split(C, dim=-1))
+        o = F.scaled_dot_product_attention(q, k, v, is_causal=True)
+        return o.transpose(1, 2).reshape(b, L, C)
+
+    def gelu_operand(self, x):
+        # through fp64: torch's fp32 CPU erf errs by several ulp near erf = -1, the kernel's erff by <= 2 ulp
+        return F.gelu(x.double()).to(self.dtype)
+
+    def token_embedding(self, tokens, table, pos):
+        vocab = table.shape[0]
+        if int(tokens.min()) < 0 or int(tokens.max()) >= vocab:
+            raise ValueError(f"token_embedding: token ids must lie in [0, {vocab})")
+        return self._c(table)[tokens] + self._c(pos)[:tokens.shape[1]]
+
     def conv3x3_direct(self, x, w_packed, bias, cout, *, stride=1, silu=False, addend=None, out_dtype=F32):
         cin = x.shape[-1]
         w = self._c(w_packed)[:, :cin, :cout].reshape(3, 3, cin, cout).permute(3, 2, 0, 1)
@@ -186,7 +203,7 @@ class TorchRefOps:
     def add_(self, x, y):
         return x.add_(y)
 
-    def cast_operand(self, x):
+    def cast_operand(self, x, weight_form=False):
         return x
 
     def softmax_rows(self, s, scale):
@@ -249,11 +266,19 @@ def _enc(x):
     return torch.cat([hi, lo, hi], dim=-1)
 
 
+def _enc_weight_form(x):
+    """operand.cuh PN_OP_SPLIT3_B: fp32 [..., C] -> bf16 [..., 3C] = [hi | hi | lo], the layout split3() packs weights in."""
+    hi = x.to(torch.bfloat16)
+    lo = (x - hi.float()).to(torch.bfloat16)
+    return torch.cat([hi, hi, lo], dim=-1)
+
+
 class TorchSplitOps(TorchRefOps):
     """CPU emulation of panacea_b200.ops.ParityOps: producers store split-bf16 operands [hi | lo | hi], weights are
     packed [W_hi | W_hi | W_lo] by the product's own split3(), and the GEMM multiplies the bf16 VALUES exactly as the
     tensor core does (bf16 x bf16 products are exact in fp32). Checks the engine's parity-mode packing/orchestration and
-    the precision claim of the encoding without a GPU."""
+    the precision claim of the encoding without a GPU. The VAE mid-block attention's operands come in both split forms:
+    the weight-form cast (pn_cast_operand mode 3) and the split3 row softmax (pn_softmax_rows_operand mode 1)."""
     operand_mult = 3
 
     def pack_matrix(self, w, taps=1):
@@ -273,8 +298,9 @@ class TorchSplitOps(TorchRefOps):
     def groupnorm_pixel(self, *a, **k):
         return _enc(super().groupnorm_pixel(*a, **k))
 
-    def layernorm(self, *a, **k):
-        return _enc(super().layernorm(*a, **k))
+    def layernorm(self, x, gamma, beta, eps=1e-5, out_f32=False):
+        y = super().layernorm(x, gamma, beta, eps)
+        return y if out_f32 else _enc(y)
 
     def attention_view(self, *a, **k):
         return _enc(super().attention_view(*a, **k))
@@ -285,6 +311,12 @@ class TorchSplitOps(TorchRefOps):
     def attention_temporal(self, *a, **k):
         return _enc(super().attention_temporal(*a, **k))
 
+    def attention_causal(self, *a, **k):
+        return _enc(super().attention_causal(*a, **k))
+
+    def gelu_operand(self, x):
+        return _enc(super().gelu_operand(x))
+
     def im2col_s2(self, x, pad=1):
         cols, geo = super().im2col_s2(x, pad)
         C = x.shape[-1]
@@ -293,5 +325,8 @@ class TorchSplitOps(TorchRefOps):
     def upsample2x(self, x):
         return _enc(super().upsample2x(x))
 
-    def cast_operand(self, x):
-        return _enc(x)
+    def cast_operand(self, x, weight_form=False):
+        return _enc_weight_form(x) if weight_form else _enc(x)
+
+    def softmax_rows(self, s, scale):
+        return _enc(super().softmax_rows(s, scale))

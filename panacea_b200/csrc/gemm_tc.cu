@@ -168,29 +168,95 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
     grow[h] = (x < p.W && y < p.H && n < p.NB) ? ((long long)n * p.H + y) * p.W + x : -1;
   }
   const int n_base = tcol * BN + 2 * quad;
+  const int n_left = p.N - n_base;                         // column block j is inside the matrix iff 8 j < n_left
+  // this thread's first element (row h, column n_base) of a row-major [rows, ld] matrix; a row outside the output
+  // (grow < 0) points at row 0 and is never dereferenced
+  auto row_at = [&](auto* base, long long ld, int h) { return base + (grow[h] < 0 ? 0 : grow[h]) * ld + n_base; };
+  const float* rv_row[2] = {p.rowvec, p.rowvec};          // row vector of each row's group
+  if (p.rowvec != nullptr) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (grow[h] >= 0) rv_row[h] += (long long)((grow[h] / p.rows_per_group) % p.n_groups) * p.ldv + n_base;
+  }
+
+  // The epilogue walks the tile in chunks of CJ column blocks. For each chunk, pass one folds every term the chunk
+  // reads into acc[] in place, one term after the other, so each element still sees bias (or the LayerNorm fold), row
+  // vector, residual, second residual in that order; pass two stores the chunk. `out` may be `residual` (in-place
+  // residual add, same leading dimension), so the compiler cannot move a load above an earlier store: stores mixed
+  // with the loads made one dependent memory round trip per 8-column block and row. Pass one has no store, and each
+  // term is straight-line code whose loads are predicated and whose adds are not (an element outside the matrix adds 0
+  // and is never stored), so a term's loads of a chunk are in flight together. The stores between chunks keep the
+  // compiler from hoisting the next chunk's loads, which bounds the registers they hold: all 80 accumulators of
+  // BN = 160 are live, and two CTAs per SM allow 128 registers per thread (CJ = 4: no spills).
+  // Reading a chunk's residuals before its stores is exact: each thread reads exactly the elements it later writes, and
+  // no other thread writes them.
+  constexpr int CJ = 4;
+  static_assert(NJ % CJ == 0, "the chunks must tile the accumulator blocks");
+  // acc[j][h] += row_h[8 j], row_h[8 j + 1] over the chunk's blocks, row_h = this thread's first element of its row h
+  // of a float or bf16 term
+  auto fold = [&](int j0, const auto* row0, const auto* row1) {
+#pragma unroll
+    for (int j = j0; j < j0 + CJ; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const auto* row = h == 0 ? row0 : row1;
+        float2 t = make_float2(0.f, 0.f);
+        if (8 * j < n_left && grow[h] >= 0) {
+          if constexpr (sizeof(*row) == 2) t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + 8 * j));
+          else t = *reinterpret_cast<const float2*>(row + 8 * j);
+        }
+        acc[4 * j + 2 * h] += t.x;
+        acc[4 * j + 2 * h + 1] += t.y;
+      }
+    }
+  };
 
   if (MODE == 2) {
     // chunk of 32 columns = 16 value columns then the 16 gate columns of the same outputs: out = value * gelu_erf(gate)
     // (reference GEGLU: attention.py:97-99, exact erf GELU). Block j (j % 4 < 2) holds values, block j + 2 their gates.
+    static_assert(CJ == 4, "a GEGLU chunk is one group of value and gate blocks");
     __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
 #pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      if ((j & 3) >= 2) continue;
-      const int n = n_base + 8 * j;
-      if (n >= p.N) continue;
-      const float2 bv = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
-      const float2 bg = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n + 16)) : make_float2(0.f, 0.f);
-      const int no = (tcol * BN) / 2 + (j >> 2) * 16 + (j & 1) * 8 + 2 * quad;
+    for (int j0 = 0; j0 < NJ; j0 += CJ) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (grow[h] < 0) continue;
-        float v0 = acc[4 * j + 2 * h] + bv.x, v1 = acc[4 * j + 2 * h + 1] + bv.y;
-        float g0 = acc[4 * (j + 2) + 2 * h] + bg.x, g1 = acc[4 * (j + 2) + 2 * h + 1] + bg.y;
-        if (p.rowvec != nullptr) {
-          const float* rv = p.rowvec + (long long)((grow[h] / p.rows_per_group) % p.n_groups) * p.ldv;
-          v0 += rv[n]; v1 += rv[n + 1]; g0 += rv[n + 16]; g1 += rv[n + 17];
+      for (int j = j0; j < j0 + 2; ++j) {
+        float2 bv = make_float2(0.f, 0.f), bg = make_float2(0.f, 0.f);
+        if (p.bias != nullptr && 8 * j < n_left) {
+          bv = __ldg(reinterpret_cast<const float2*>(p.bias + n_base + 8 * j));
+          bg = __ldg(reinterpret_cast<const float2*>(p.bias + n_base + 8 * j + 16));
         }
-        *reinterpret_cast<uint32_t*>(out + grow[h] * p.ldo + no) = pack_bf16x2(geglu_f32(v0, g0), geglu_f32(v1, g1));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          acc[4 * j + 2 * h] += bv.x; acc[4 * j + 2 * h + 1] += bv.y;
+          acc[4 * (j + 2) + 2 * h] += bg.x; acc[4 * (j + 2) + 2 * h + 1] += bg.y;
+        }
+      }
+      if (p.rowvec != nullptr) {
+#pragma unroll
+        for (int j = j0; j < j0 + 2; ++j) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (8 * j < n_left && grow[h] >= 0) {
+              const float* rv = rv_row[h] + 8 * j;
+              t = make_float4(rv[0], rv[1], rv[16], rv[17]);
+            }
+            acc[4 * j + 2 * h] += t.x; acc[4 * j + 2 * h + 1] += t.y;
+            acc[4 * (j + 2) + 2 * h] += t.z; acc[4 * (j + 2) + 2 * h + 1] += t.w;
+          }
+        }
+      }
+#pragma unroll
+      for (int j = j0; j < j0 + 2; ++j) {
+        if (8 * j >= n_left) continue;
+        const int no = (tcol * BN) / 2 + (j >> 2) * 16 + (j & 1) * 8 + 2 * quad;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (grow[h] < 0) continue;
+          *reinterpret_cast<uint32_t*>(out + grow[h] * p.ldo + no) =
+              pack_bf16x2(geglu_f32(acc[4 * j + 2 * h], acc[4 * (j + 2) + 2 * h]),
+                          geglu_f32(acc[4 * j + 2 * h + 1], acc[4 * (j + 2) + 2 * h + 1]));
+        }
       }
     }
     return;
@@ -212,50 +278,55 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
   }
   float st_sum[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, st_sq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][column half]
 #pragma unroll
-  for (int j = 0; j < NJ; ++j) {
-    const int n = n_base + 8 * j;
-    if (n >= p.N) continue;
-    const float2 b2 = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
-    float2 s2 = make_float2(0.f, 0.f);
-    if (MODE == 1 && p.ln_stats_in != nullptr) s2 = __ldg(reinterpret_cast<const float2*>(p.ln_colsum + n));
+  for (int j0 = 0; j0 < NJ; j0 += CJ) {
+    // pass one
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      if (grow[h] < 0) continue;
-      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-      if (MODE == 1 && p.ln_stats_in != nullptr) {
-        v0 = fmaf(ln_a[h], v0, fmaf(ln_b[h], s2.x, b2.x));
-        v1 = fmaf(ln_a[h], v1, fmaf(ln_b[h], s2.y, b2.y));
-      } else {
-        v0 += b2.x; v1 += b2.y;
-      }
-      if (p.rowvec != nullptr) {
-        const float2 r2 = __ldg(reinterpret_cast<const float2*>(
-            p.rowvec + (long long)((grow[h] / p.rows_per_group) % p.n_groups) * p.ldv + n));
-        v0 += r2.x; v1 += r2.y;
-      }
-      if (p.residual != nullptr) {
-        if (MODE == 1 && p.res_bf16) {
-          const float2 r2 = __bfloat1622float2(
-              *reinterpret_cast<const __nv_bfloat162*>(reinterpret_cast<const __nv_bfloat16*>(p.residual) + grow[h] * p.ldr + n));
-          v0 += r2.x; v1 += r2.y;
+    for (int j = j0; j < j0 + CJ; ++j) {
+      float2 b2 = make_float2(0.f, 0.f), s2 = make_float2(0.f, 0.f);
+      if (p.bias != nullptr && 8 * j < n_left) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + n_base + 8 * j));
+      if (MODE == 1 && p.ln_stats_in != nullptr && 8 * j < n_left)
+        s2 = __ldg(reinterpret_cast<const float2*>(p.ln_colsum + n_base + 8 * j));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float &v0 = acc[4 * j + 2 * h], &v1 = acc[4 * j + 2 * h + 1];
+        if (MODE == 1 && p.ln_stats_in != nullptr) {
+          v0 = fmaf(ln_a[h], v0, fmaf(ln_b[h], s2.x, b2.x));
+          v1 = fmaf(ln_a[h], v1, fmaf(ln_b[h], s2.y, b2.y));
         } else {
-          const float2 r2 = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.residual) + grow[h] * p.ldr + n);
-          v0 += r2.x; v1 += r2.y;
+          v0 += b2.x; v1 += b2.y;
         }
       }
-      if (MODE == 0) {
-        if (p.residual2 != nullptr) {
-          const float2 r2 = *reinterpret_cast<const float2*>(p.residual2 + grow[h] * p.ldr2 + n);
-          v0 += r2.x; v1 += r2.y;
-        }
-        *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + grow[h] * p.ldo + n) = make_float2(v0, v1);
+    }
+    if (p.rowvec != nullptr) fold(j0, rv_row[0], rv_row[1]);
+    if (p.residual != nullptr) {
+      if (MODE == 1 && p.res_bf16) {
+        const __nv_bfloat16* res = reinterpret_cast<const __nv_bfloat16*>(p.residual);
+        fold(j0, row_at(res, p.ldr, 0), row_at(res, p.ldr, 1));
       } else {
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + grow[h] * p.ldo + n) = pack_bf16x2(v0, v1);
-        // row sums of the fp32 values (their bf16 rounding, which the consumer's MMA reads, perturbs mean / variance
-        // by < 2^-9 / sqrt(C))
-        const int hf = j < NJ / 2 ? 0 : 1;
-        st_sum[h][hf] += v0 + v1;
-        st_sq[h][hf] = fmaf(v0, v0, fmaf(v1, v1, st_sq[h][hf]));
+        const float* res = reinterpret_cast<const float*>(p.residual);
+        fold(j0, row_at(res, p.ldr, 0), row_at(res, p.ldr, 1));
+      }
+    }
+    if (MODE == 0 && p.residual2 != nullptr) fold(j0, row_at(p.residual2, p.ldr2, 0), row_at(p.residual2, p.ldr2, 1));
+
+    // pass two
+#pragma unroll
+    for (int j = j0; j < j0 + CJ; ++j) {
+      if (8 * j >= n_left) continue;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (grow[h] < 0) continue;
+        const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (MODE == 0) {
+          *reinterpret_cast<float2*>(row_at(reinterpret_cast<float*>(p.out), p.ldo, h) + 8 * j) = make_float2(v0, v1);
+        } else {
+          *reinterpret_cast<uint32_t*>(row_at(reinterpret_cast<__nv_bfloat16*>(p.out), p.ldo, h) + 8 * j) = pack_bf16x2(v0, v1);
+          // row sums of the fp32 values (their bf16 rounding, which the consumer's MMA reads, perturbs mean / variance
+          // by < 2^-9 / sqrt(C))
+          const int hf = j < NJ / 2 ? 0 : 1;
+          st_sum[h][hf] += v0 + v1;
+          st_sq[h][hf] = fmaf(v0, v0, fmaf(v1, v1, st_sq[h][hf]));
+        }
       }
     }
   }

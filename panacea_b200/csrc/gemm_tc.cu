@@ -22,7 +22,7 @@
 // addressing) and <= 114 KB of shared memory per CTA (3 stages at BN = 160).
 // Pipeline: STAGES-deep full/empty mbarrier ring; a stage is handed back once the wgmma group that read it retired.
 #include "common.cuh"
-#include "ptx.cuh"
+#include "gemm_epilogue.cuh"
 #include "../../include/panacea_b200.h"
 
 namespace pn {
@@ -33,38 +33,10 @@ constexpr int SM_SMEM_BYTES = 233472;      // 228 KB of shared memory per H100 S
 constexpr int CTA_SMEM_RESERVED = 1024;    // ... of which the system reserves 1 KB per resident CTA
 constexpr int GEMM_THREADS = 256;
 constexpr int GEMM_CTAS_PER_SM = 2;
-
-struct GemmParams {
-  CUtensorMap mapA;
-  CUtensorMap mapB;
-  // geometry of the A tensor / output rows
-  int NB, H, W;
-  int tw, th, tn;             // tile box extents, tw*th*tn == 128
-  int tiles_w, tiles_h, tiles_n, tiles_col;
-  int kc_per_tap;             // C / 64
-  int taps_h, taps_w, pad_h, pad_w;
-  int N;                      // GEMM N (weight rows)
-  // epilogue
-  void* out;
-  const float* bias;
-  const float* rowvec;
-  const void* residual;
-  const float* residual2;
-  long long ldo, ldr, ldr2, ldv;
-  int rows_per_group, n_groups;
-  // LayerNorm folded into the GEMMs around the bf16 token stream (attention.py:726-747: x + attn(norm(x))):
-  //  * a PRODUCER of the stream also emits per-row partial sums (sum, sum of squares) of the values it stores:
-  //    ln_stats_out[row][tile_col * 2 + half][2] (ln_parts_out = 2 * tiles_col, half = which half of the tile's columns);
-  //  * a CONSUMER multiplies the UN-normalised stream by W' = W diag(gamma) and finishes the LayerNorm in its
-  //    epilogue: out = rstd_m * (acc - mean_m * s_n) + t_n, s_n = sum_k W'[n,k], t_n = sum_k beta_k W[n,k] (+ bias,
-  //    passed as `bias`), mean/rstd from the ln_parts_in partial sums of row m.
-  const float* ln_stats_in;
-  const float* ln_colsum;
-  float* ln_stats_out;
-  int ln_parts_in, ln_parts_out;
-  float ln_inv_dim, ln_eps;
-  int res_bf16;                // the residual is bf16 (bf16 token stream of the transformer blocks), bf16 output only
-};
+// Fewest rows for which pn_gemm runs an eligible 1x1 GEMM on gemm_ws.cu's persistent kernel. With an fp32 residual at
+// K = 320 (H100 80GB HBM3, 700 W) it took 7.4 / 7.9 us at 512 rows and N = 320 / 1280, against gemm_tc_kernel's 8.5 / 8.7;
+// the 16-row time-embedding linear stays on gemm_tc_kernel.
+constexpr long long WS_MIN_ROWS = 512;
 
 template <int BN, int STAGES>
 struct GemmSmem {
@@ -205,8 +177,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
           if constexpr (sizeof(*row) == 2) t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + 8 * j));
           else t = *reinterpret_cast<const float2*>(row + 8 * j);
         }
-        acc[4 * j + 2 * h] += t.x;
-        acc[4 * j + 2 * h + 1] += t.y;
+        epi_add(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], t);
       }
     }
   };
@@ -227,8 +198,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          acc[4 * j + 2 * h] += bv.x; acc[4 * j + 2 * h + 1] += bv.y;
-          acc[4 * (j + 2) + 2 * h] += bg.x; acc[4 * (j + 2) + 2 * h + 1] += bg.y;
+          epi_add(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], bv);
+          epi_add(acc[4 * (j + 2) + 2 * h], acc[4 * (j + 2) + 2 * h + 1], bg);
         }
       }
       if (p.rowvec != nullptr) {
@@ -241,8 +212,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
               const float* rv = rv_row[h] + 8 * j;
               t = make_float4(rv[0], rv[1], rv[16], rv[17]);
             }
-            acc[4 * j + 2 * h] += t.x; acc[4 * j + 2 * h + 1] += t.y;
-            acc[4 * (j + 2) + 2 * h] += t.z; acc[4 * (j + 2) + 2 * h + 1] += t.w;
+            epi_add(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], make_float2(t.x, t.y));
+            epi_add(acc[4 * (j + 2) + 2 * h], acc[4 * (j + 2) + 2 * h + 1], make_float2(t.z, t.w));
           }
         }
       }
@@ -266,14 +237,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
   if (MODE == 1 && p.ln_stats_in != nullptr) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      if (grow[h] < 0) continue;
-      float sm = 0.f, sq = 0.f;
-      const float2* st = reinterpret_cast<const float2*>(p.ln_stats_in) + grow[h] * p.ln_parts_in;
-      for (int q = 0; q < p.ln_parts_in; ++q) { const float2 t2 = __ldg(st + q); sm += t2.x; sq += t2.y; }
-      const float mu = sm * p.ln_inv_dim;
-      const float rstd = rsqrtf(fmaxf(sq * p.ln_inv_dim - mu * mu, 0.f) + p.ln_eps);
-      ln_a[h] = rstd;
-      ln_b[h] = -rstd * mu;
+      if (grow[h] >= 0) ln_row_coeffs(p, grow[h], ln_a[h], ln_b[h]);
     }
   }
   float st_sum[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, st_sq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][column half]
@@ -287,15 +251,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
       if (MODE == 1 && p.ln_stats_in != nullptr && 8 * j < n_left)
         s2 = __ldg(reinterpret_cast<const float2*>(p.ln_colsum + n_base + 8 * j));
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float &v0 = acc[4 * j + 2 * h], &v1 = acc[4 * j + 2 * h + 1];
-        if (MODE == 1 && p.ln_stats_in != nullptr) {
-          v0 = fmaf(ln_a[h], v0, fmaf(ln_b[h], s2.x, b2.x));
-          v1 = fmaf(ln_a[h], v1, fmaf(ln_b[h], s2.y, b2.y));
-        } else {
-          v0 += b2.x; v1 += b2.y;
-        }
-      }
+      for (int h = 0; h < 2; ++h)
+        epi_bias(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b2, s2, MODE == 1 && p.ln_stats_in != nullptr, ln_a[h], ln_b[h]);
     }
     if (p.rowvec != nullptr) fold(j0, rv_row[0], rv_row[1]);
     if (p.residual != nullptr) {
@@ -321,11 +278,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
           *reinterpret_cast<float2*>(row_at(reinterpret_cast<float*>(p.out), p.ldo, h) + 8 * j) = make_float2(v0, v1);
         } else {
           *reinterpret_cast<uint32_t*>(row_at(reinterpret_cast<__nv_bfloat16*>(p.out), p.ldo, h) + 8 * j) = pack_bf16x2(v0, v1);
-          // row sums of the fp32 values (their bf16 rounding, which the consumer's MMA reads, perturbs mean / variance
-          // by < 2^-9 / sqrt(C))
           const int hf = j < NJ / 2 ? 0 : 1;
-          st_sum[h][hf] += v0 + v1;
-          st_sq[h][hf] = fmaf(v0, v0, fmaf(v1, v1, st_sq[h][hf]));
+          row_stats_add(st_sum[h][hf], st_sq[h][hf], v0, v1);
         }
       }
     }
@@ -335,9 +289,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
     for (int h = 0; h < 2; ++h) {
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {
-        float s = st_sum[h][hf], q = st_sq[h][hf];
-        s += __shfl_xor_sync(0xffffffffu, s, 1); s += __shfl_xor_sync(0xffffffffu, s, 2);
-        q += __shfl_xor_sync(0xffffffffu, q, 1); q += __shfl_xor_sync(0xffffffffu, q, 2);
+        const float s = quad_sum(st_sum[h][hf]), q = quad_sum(st_sq[h][hf]);
         if (quad == 0 && grow[h] >= 0)
           reinterpret_cast<float2*>(p.ln_stats_out)[grow[h] * p.ln_parts_out + tcol * 2 + hf] = make_float2(s, q);
       }
@@ -447,20 +399,26 @@ extern "C" int pn_gemm(const pn_gemm_args* a, void* stream_v) {
   const long long tiles = (long long)p.tiles_w * p.tiles_h * p.tiles_n * p.tiles_col;
   PN_REQUIRE(tiles > 0 && tiles < (1ll << 31), "pn_gemm: too many output tiles");
 
-  const uint64_t dimsA[4] = {(uint64_t)a->C, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
-  const uint64_t strA[3] = {(uint64_t)sw, (uint64_t)sh, (uint64_t)sn};
-  const uint32_t boxA[4] = {64u, (uint32_t)tw, (uint32_t)th, (uint32_t)tn};
-  int rc = cached_tmap_bf16(&p.mapA, a->A, 4, dimsA, strA, boxA, 128);
-  if (rc != PN_OK) return rc;
   const uint64_t K = (uint64_t)a->taps_h * a->taps_w * a->C;
   const uint64_t dimsB[2] = {K, (uint64_t)a->N};
   const uint64_t strB[1] = {K};
   const uint32_t boxB[2] = {64u, (uint32_t)BN};
-  rc = cached_tmap_bf16(&p.mapB, a->B, 2, dimsB, strB, boxB, 128);
+  int rc = cached_tmap_bf16(&p.mapB, a->B, 2, dimsB, strB, boxB, 128);
   if (rc != PN_OK) return rc;
-
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   const int mode = a->geglu ? 2 : a->out_bf16 ? 1 : 0;
+
+  // 1x1 GEMMs over many dense rows whose 160 x K weight tile fits in shared memory (the level-0 linears, K = 320): the
+  // persistent weight-stationary kernel of gemm_ws.cu. Its TMA maps over the residual need a 16-byte aligned base.
+  if (pointwise && NB == 1 && H == 1 && a->C <= 320 && a->N % 160 == 0 && W >= WS_MIN_ROWS &&
+      p.tiles_col <= sm_count() && (reinterpret_cast<uintptr_t>(a->residual) & 15) == 0)
+    return launch_gemm_ws(p, mode, a->A, W, sw, (int)a->C, stream);
+
+  const uint64_t dimsA[4] = {(uint64_t)a->C, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
+  const uint64_t strA[3] = {(uint64_t)sw, (uint64_t)sh, (uint64_t)sn};
+  const uint32_t boxA[4] = {64u, (uint32_t)tw, (uint32_t)th, (uint32_t)tn};
+  rc = cached_tmap_bf16(&p.mapA, a->A, 4, dimsA, strA, boxA, 128);
+  if (rc != PN_OK) return rc;
   switch (BN) {
     // the deepest rings that still fit two CTAs per SM (111,664 / 99,376 / 99,392 / 103,504 bytes per CTA)
     case 160: return launch_gemm<160, 3>(p, mode, tiles, stream);

@@ -115,6 +115,20 @@ __device__ __forceinline__ void tma_load_stage_if(bool pred, uint64_t* bar, uint
       "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(smem_u32(dst_b)), "l"(reinterpret_cast<uint64_t>(map_b)), "r"(b0), "r"(b1)
       : "memory");
 }
+// shared -> global tile store, tracked by the issuing thread's bulk async-groups
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// this thread's bulk stores have finished reading their shared-memory source
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// ... and their global writes are complete
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// barrier `id` (1..15) over `threads` threads of the CTA
+__device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
                                             int c2, int c3, int c4) {
   asm volatile(

@@ -46,9 +46,7 @@ struct GemmSmem {
   static constexpr int TOTAL = STAGES * STAGE_BYTES + 2 * STAGES * 8 + 1024;
 };
 
-// MODE: 0 = fp32 store (+ fp32 residual, + second fp32 residual), 1 = bf16 store (+ fp32 or bf16 residual, LayerNorm
-// fold / row statistics), 2 = GEGLU (bf16 store of N/2 columns)
-template <int BN, int STAGES, int MODE>
+template <int BN, int STAGES, int MODE>    // MODE: an EpiMode
 __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   using S = GemmSmem<BN, STAGES>;
   constexpr int NJ = BN / 8;                   // 8-column accumulator blocks per thread row
@@ -144,12 +142,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
   // this thread's first element (row h, column n_base) of a row-major [rows, ld] matrix; a row outside the output
   // (grow < 0) points at row 0 and is never dereferenced
   auto row_at = [&](auto* base, long long ld, int h) { return base + (grow[h] < 0 ? 0 : grow[h]) * ld + n_base; };
-  const float* rv_row[2] = {p.rowvec, p.rowvec};          // row vector of each row's group
-  if (p.rowvec != nullptr) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-      if (grow[h] >= 0) rv_row[h] += (long long)((grow[h] / p.rows_per_group) % p.n_groups) * p.ldv + n_base;
-  }
+  const float* rv_row[2];
+  rowvec_rows(p, grow, n_base, rv_row);
 
   // The epilogue walks the tile in chunks of CJ column blocks. For each chunk, pass one folds every term the chunk
   // reads into acc[] in place, one term after the other, so each element still sees bias (or the LayerNorm fold), row
@@ -182,9 +176,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
     }
   };
 
-  if (MODE == 2) {
-    // chunk of 32 columns = 16 value columns then the 16 gate columns of the same outputs: out = value * gelu_erf(gate)
-    // (reference GEGLU: attention.py:97-99, exact erf GELU). Block j (j % 4 < 2) holds values, block j + 2 their gates.
+  if (MODE == EPI_GEGLU) {
     static_assert(CJ == 4, "a GEGLU chunk is one group of value and gate blocks");
     __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
 #pragma unroll
@@ -197,10 +189,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
           bg = __ldg(reinterpret_cast<const float2*>(p.bias + n_base + 8 * j + 16));
         }
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          epi_add(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], bv);
-          epi_add(acc[4 * (j + 2) + 2 * h], acc[4 * (j + 2) + 2 * h + 1], bg);
-        }
+        for (int h = 0; h < 2; ++h) geglu_add(acc, j, h, bv, bg);
       }
       if (p.rowvec != nullptr) {
 #pragma unroll
@@ -212,29 +201,24 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
               const float* rv = rv_row[h] + 8 * j;
               t = make_float4(rv[0], rv[1], rv[16], rv[17]);
             }
-            epi_add(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], make_float2(t.x, t.y));
-            epi_add(acc[4 * (j + 2) + 2 * h], acc[4 * (j + 2) + 2 * h + 1], make_float2(t.z, t.w));
+            geglu_add(acc, j, h, make_float2(t.x, t.y), make_float2(t.z, t.w));
           }
         }
       }
 #pragma unroll
       for (int j = j0; j < j0 + 2; ++j) {
         if (8 * j >= n_left) continue;
-        const int no = (tcol * BN) / 2 + (j >> 2) * 16 + (j & 1) * 8 + 2 * quad;
+        const int no = (tcol * BN) / 2 + geglu_out_col(j, quad);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (grow[h] < 0) continue;
-          *reinterpret_cast<uint32_t*>(out + grow[h] * p.ldo + no) =
-              pack_bf16x2(geglu_f32(acc[4 * j + 2 * h], acc[4 * (j + 2) + 2 * h]),
-                          geglu_f32(acc[4 * j + 2 * h + 1], acc[4 * (j + 2) + 2 * h + 1]));
-        }
+        for (int h = 0; h < 2; ++h)
+          if (grow[h] >= 0) *reinterpret_cast<uint32_t*>(out + grow[h] * p.ldo + no) = geglu_out(acc, j, h);
       }
     }
     return;
   }
 
   float ln_a[2] = {1.f, 1.f}, ln_b[2] = {0.f, 0.f};       // folded LayerNorm: out = a * acc + b * s_n + t_n
-  if (MODE == 1 && p.ln_stats_in != nullptr) {
+  if (MODE == EPI_BF16 && p.ln_stats_in != nullptr) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (grow[h] >= 0) ln_row_coeffs(p, grow[h], ln_a[h], ln_b[h]);
@@ -248,15 +232,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
     for (int j = j0; j < j0 + CJ; ++j) {
       float2 b2 = make_float2(0.f, 0.f), s2 = make_float2(0.f, 0.f);
       if (p.bias != nullptr && 8 * j < n_left) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + n_base + 8 * j));
-      if (MODE == 1 && p.ln_stats_in != nullptr && 8 * j < n_left)
+      if (MODE == EPI_BF16 && p.ln_stats_in != nullptr && 8 * j < n_left)
         s2 = __ldg(reinterpret_cast<const float2*>(p.ln_colsum + n_base + 8 * j));
 #pragma unroll
       for (int h = 0; h < 2; ++h)
-        epi_bias(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b2, s2, MODE == 1 && p.ln_stats_in != nullptr, ln_a[h], ln_b[h]);
+        epi_bias(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b2, s2, MODE == EPI_BF16 && p.ln_stats_in != nullptr, ln_a[h], ln_b[h]);
     }
     if (p.rowvec != nullptr) fold(j0, rv_row[0], rv_row[1]);
     if (p.residual != nullptr) {
-      if (MODE == 1 && p.res_bf16) {
+      if (MODE == EPI_BF16 && p.res_bf16) {
         const __nv_bfloat16* res = reinterpret_cast<const __nv_bfloat16*>(p.residual);
         fold(j0, row_at(res, p.ldr, 0), row_at(res, p.ldr, 1));
       } else {
@@ -264,7 +248,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
         fold(j0, row_at(res, p.ldr, 0), row_at(res, p.ldr, 1));
       }
     }
-    if (MODE == 0 && p.residual2 != nullptr) fold(j0, row_at(p.residual2, p.ldr2, 0), row_at(p.residual2, p.ldr2, 1));
+    if (MODE == EPI_F32 && p.residual2 != nullptr) fold(j0, row_at(p.residual2, p.ldr2, 0), row_at(p.residual2, p.ldr2, 1));
 
     // pass two
 #pragma unroll
@@ -274,27 +258,16 @@ __global__ void __launch_bounds__(GEMM_THREADS, GEMM_CTAS_PER_SM) gemm_tc_kernel
       for (int h = 0; h < 2; ++h) {
         if (grow[h] < 0) continue;
         const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (MODE == 0) {
+        if (MODE == EPI_F32) {
           *reinterpret_cast<float2*>(row_at(reinterpret_cast<float*>(p.out), p.ldo, h) + 8 * j) = make_float2(v0, v1);
         } else {
           *reinterpret_cast<uint32_t*>(row_at(reinterpret_cast<__nv_bfloat16*>(p.out), p.ldo, h) + 8 * j) = pack_bf16x2(v0, v1);
-          const int hf = j < NJ / 2 ? 0 : 1;
-          row_stats_add(st_sum[h][hf], st_sq[h][hf], v0, v1);
+          row_stats_add<NJ>(st_sum, st_sq, h, j, v0, v1);
         }
       }
     }
   }
-  if (MODE == 1 && p.ln_stats_out != nullptr) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-#pragma unroll
-      for (int hf = 0; hf < 2; ++hf) {
-        const float s = quad_sum(st_sum[h][hf]), q = quad_sum(st_sq[h][hf]);
-        if (quad == 0 && grow[h] >= 0)
-          reinterpret_cast<float2*>(p.ln_stats_out)[grow[h] * p.ln_parts_out + tcol * 2 + hf] = make_float2(s, q);
-      }
-    }
-  }
+  if (MODE == EPI_BF16 && p.ln_stats_out != nullptr) row_stats_store(p, st_sum, st_sq, grow, tcol, quad);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -316,18 +289,22 @@ static void pick_tile(long long NB, long long H, long long W, int* tw, int* th, 
 }
 
 template <int BN, int STAGES>
-static int launch_gemm(const GemmParams& p, int mode, long long tiles, cudaStream_t stream) {
+static int launch_gemm(const GemmParams& p, EpiMode mode, long long tiles, cudaStream_t stream) {
   using S = GemmSmem<BN, STAGES>;
   static_assert(GEMM_CTAS_PER_SM * (S::TOTAL + CTA_SMEM_RESERVED) <= SM_SMEM_BYTES,
                 "shared memory budget exceeded: two CTAs must fit one SM");
-  void (*kern)(GemmParams) = mode == 2 ? gemm_tc_kernel<BN, STAGES, 2> : mode == 1 ? gemm_tc_kernel<BN, STAGES, 1>
-                                                                                   : gemm_tc_kernel<BN, STAGES, 0>;
+  void (*kern)(GemmParams) = mode == EPI_GEGLU ? gemm_tc_kernel<BN, STAGES, EPI_GEGLU>
+                             : mode == EPI_BF16 ? gemm_tc_kernel<BN, STAGES, EPI_BF16> : gemm_tc_kernel<BN, STAGES, EPI_F32>;
   const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), S::TOTAL, /*max_carveout=*/true);
   if (rc != PN_OK) return rc;
   kern<<<(unsigned)tiles, GEMM_THREADS, S::TOTAL, stream>>>(p);
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
+
+// Column-tile width of a GEMM with N output columns. Every channel count of the network is a multiple of 160
+// (320/640/960/1280/1920/2560/5120/10240); a 128 x 160 fp32 accumulator is 80 registers per consumer thread.
+static int gemm_bn(int N) { return N % 160 == 0 ? 160 : N >= 128 ? 128 : N > 32 ? 64 : 32; }
 
 }  // namespace pn
 
@@ -387,9 +364,7 @@ extern "C" int pn_gemm(const pn_gemm_args* a, void* stream_v) {
   p.ln_stats_in = a->ln_stats_in; p.ln_colsum = a->ln_colsum; p.ln_stats_out = a->ln_stats_out;
   p.ln_parts_in = a->ln_parts_in; p.ln_eps = a->ln_eps; p.ln_inv_dim = 1.0f / (float)a->C;
 
-  // N tile: every channel count of the network is a multiple of 160 (320/640/960/1280/1920/2560/5120/10240); a
-  // 128 x 160 fp32 accumulator is 80 registers per consumer thread.
-  const int BN = a->N % 160 == 0 ? 160 : a->N >= 128 ? 128 : a->N > 32 ? 64 : 32;
+  const int BN = gemm_bn(a->N);
   p.tiles_col = (a->N + BN - 1) / BN;
   if (a->ln_stats_out) {
     PN_REQUIRE(a->out_bf16 && !a->geglu && a->ln_stats_in == nullptr && pn_gemm_ln_parts(a->N) == 2 * p.tiles_col,
@@ -406,7 +381,7 @@ extern "C" int pn_gemm(const pn_gemm_args* a, void* stream_v) {
   int rc = cached_tmap_bf16(&p.mapB, a->B, 2, dimsB, strB, boxB, 128);
   if (rc != PN_OK) return rc;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-  const int mode = a->geglu ? 2 : a->out_bf16 ? 1 : 0;
+  const EpiMode mode = a->geglu ? EPI_GEGLU : a->out_bf16 ? EPI_BF16 : EPI_F32;
 
   // 1x1 GEMMs over many dense rows whose 160 x K weight tile fits in shared memory (the level-0 linears, K = 320): the
   // persistent weight-stationary kernel of gemm_ws.cu. Its TMA maps over the residual need a 16-byte aligned base.
@@ -431,7 +406,5 @@ extern "C" int pn_gemm(const pn_gemm_args* a, void* stream_v) {
 // number of partial (sum, sum of squares) pairs per row that a bf16 pn_gemm with N output columns writes to
 // ln_stats_out (2 per 160- or 128-wide column tile)
 extern "C" int pn_gemm_ln_parts(int N) {
-  if (N <= 0 || (N % 160 != 0 && N % 128 != 0)) return 0;
-  const int BN = (N % 160 == 0) ? 160 : 128;
-  return 2 * (N / BN);
+  return N > 0 && (N % 160 == 0 || N % 128 == 0) ? 2 * (N / gemm_bn(N)) : 0;
 }

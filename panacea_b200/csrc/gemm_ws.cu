@@ -62,9 +62,7 @@ struct GemmWsParams {
   int M, row_tiles, groups, kc;
 };
 
-// MODE as gemm_tc_kernel: 0 = fp32 store (+ fp32 residual, + second fp32 residual), 1 = bf16 store (+ fp32 or bf16
-// residual, LayerNorm fold / row statistics), 2 = GEGLU
-template <int MODE>
+template <int MODE>    // MODE: an EpiMode
 __global__ void __launch_bounds__(WS_THREADS, 1) gemm_ws_kernel(const __grid_constant__ GemmWsParams q) {
   const GemmParams& p = q.p;
   constexpr int NJ = WS_BN / 8;
@@ -86,9 +84,9 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gemm_ws_kernel(const __grid_con
   const int lane = threadIdx.x & 31;
   const int col = blockIdx.x % p.tiles_col;
   const int grp = blockIdx.x / p.tiles_col;
-  const bool has_res = MODE != 2 && p.residual != nullptr;
-  const bool res_bf16 = MODE == 1 && p.res_bf16;
-  const bool ln = MODE == 1 && p.ln_stats_in != nullptr;
+  const bool has_res = MODE != EPI_GEGLU && p.residual != nullptr;
+  const bool res_bf16 = MODE == EPI_BF16 && p.res_bf16;
+  const bool ln = MODE == EPI_BF16 && p.ln_stats_in != nullptr;
 
   // The column vectors are the same for every row tile of the CTA. Read in the epilogue straight from global memory,
   // under the kernel's own HBM traffic, they cost a memory round trip per tile.
@@ -220,25 +218,17 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gemm_ws_kernel(const __grid_con
       const long long row = (long long)rt * WS_BM + r0 + 8 * h;
       grow[h] = row < q.M ? row : -1;
     }
-    const float* rv_row[2] = {p.rowvec, p.rowvec};
-    if (p.rowvec != nullptr) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-        if (grow[h] >= 0) rv_row[h] += (long long)((grow[h] / p.rows_per_group) % p.n_groups) * p.ldv + n_base;
-    }
+    const float* rv_row[2];
+    rowvec_rows(p, grow, n_base, rv_row);
 
-    if (MODE == 2) {
-      // block j (j % 4 < 2) holds values, block j + 2 their gates
+    if (MODE == EPI_GEGLU) {
 #pragma unroll
       for (int j = 0; j < NJ; ++j) {
         if ((j & 3) >= 2) continue;
         const float2 bv = *reinterpret_cast<const float2*>(s_bias + 2 * quad + 8 * j);
         const float2 bg = *reinterpret_cast<const float2*>(s_bias + 2 * quad + 8 * j + 16);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          epi_add(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], bv);
-          epi_add(acc[4 * (j + 2) + 2 * h], acc[4 * (j + 2) + 2 * h + 1], bg);
-        }
+        for (int h = 0; h < 2; ++h) geglu_add(acc, j, h, bv, bg);
       }
       if (p.rowvec != nullptr) {
 #pragma unroll
@@ -246,13 +236,12 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gemm_ws_kernel(const __grid_con
           if ((j & 3) >= 2) continue;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            float4 t4 = make_float4(0.f, 0.f, 0.f, 0.f);
+            float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
             if (grow[h] >= 0) {
               const float* rv = rv_row[h] + 8 * j;
-              t4 = make_float4(rv[0], rv[1], rv[16], rv[17]);
+              t = make_float4(rv[0], rv[1], rv[16], rv[17]);
             }
-            epi_add(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], make_float2(t4.x, t4.y));
-            epi_add(acc[4 * (j + 2) + 2 * h], acc[4 * (j + 2) + 2 * h + 1], make_float2(t4.z, t4.w));
+            geglu_add(acc, j, h, make_float2(t.x, t.y), make_float2(t.z, t.w));
           }
         }
       }
@@ -261,12 +250,9 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gemm_ws_kernel(const __grid_con
 #pragma unroll
       for (int j = 0; j < NJ; ++j) {
         if ((j & 3) >= 2) continue;
-        const int oc = (j >> 2) * 16 + (j & 1) * 8 + 2 * quad;
 #pragma unroll
         for (int h = 0; h < 2; ++h)
-          *reinterpret_cast<uint32_t*>(stg + stage_off<32>(r0 + 8 * h, 2 * oc)) =
-              pack_bf16x2(geglu_f32(acc[4 * j + 2 * h], acc[4 * (j + 2) + 2 * h]),
-                          geglu_f32(acc[4 * j + 2 * h + 1], acc[4 * (j + 2) + 2 * h + 1]));
+          *reinterpret_cast<uint32_t*>(stg + stage_off<32>(r0 + 8 * h, 2 * geglu_out_col(j, quad))) = geglu_out(acc, j, h);
       }
       fence_proxy_async_smem();
       named_barrier_sync(1 + wg, 128);
@@ -308,7 +294,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gemm_ws_kernel(const __grid_con
           epi_add(v0, v1, res_bf16 ? __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(stg + stage_off<64>(r, 2 * c)))
                                    : *reinterpret_cast<const float2*>(stg + stage_off<128>(r, 4 * c)));
         }
-        if (MODE == 0 && p.residual2 != nullptr) {
+        if (MODE == EPI_F32 && p.residual2 != nullptr) {
           float2 t2 = make_float2(0.f, 0.f);
           if (grow[h] >= 0) t2 = *reinterpret_cast<const float2*>(p.residual2 + grow[h] * p.ldr2 + n_base + 8 * j);
           epi_add(v0, v1, t2);
@@ -326,17 +312,17 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gemm_ws_kernel(const __grid_con
       for (int h = 0; h < 2; ++h) {
         const int r = r0 + 8 * h, c = 8 * j + 2 * quad;
         const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (MODE == 0) {
+        if (MODE == EPI_F32) {
           *reinterpret_cast<float2*>(stg + stage_off<128>(r, 4 * c)) = make_float2(v0, v1);
         } else {
           *reinterpret_cast<uint32_t*>(stg + stage_off<64>(r, 2 * c)) = pack_bf16x2(v0, v1);
-          row_stats_add(st_sum[h][j < NJ / 2 ? 0 : 1], st_sq[h][j < NJ / 2 ? 0 : 1], v0, v1);
+          row_stats_add<NJ>(st_sum, st_sq, h, j, v0, v1);
         }
       }
     fence_proxy_async_smem();
     named_barrier_sync(1 + wg, 128);
     if (issuer) {
-      const int box = MODE == 0 ? WS_BM * 128 : WS_BM * 64;
+      const int box = MODE == EPI_F32 ? WS_BM * 128 : WS_BM * 64;
       for (int b = 0; b < WS_BN / 32; ++b) tma_store_2d(&q.mapOut, stg + b * box, col * WS_BN + 32 * b, rt * WS_BM);
       bulk_commit();
       if (has_res) {                                    // hand the staging buffer back for this warpgroup's next residual
@@ -344,21 +330,12 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gemm_ws_kernel(const __grid_con
         mbar_arrive(&res_empty[wg]);
       }
     }
-    if (MODE == 1 && p.ln_stats_out != nullptr) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          const float s = quad_sum(st_sum[h][hf]), sq = quad_sum(st_sq[h][hf]);
-          if (quad == 0 && grow[h] >= 0)
-            reinterpret_cast<float2*>(p.ln_stats_out)[grow[h] * p.ln_parts_out + col * 2 + hf] = make_float2(s, sq);
-        }
-    }
+    if (MODE == EPI_BF16 && p.ln_stats_out != nullptr) row_stats_store(p, st_sum, st_sq, grow, col, quad);
   }
   if (issuer) bulk_wait_all();
 }
 
-int launch_gemm_ws(GemmParams& p, int mode, const void* A, long long rows, long long row_stride, int C, cudaStream_t stream) {
+int launch_gemm_ws(GemmParams& p, EpiMode mode, const void* A, long long rows, long long row_stride, int C, cudaStream_t stream) {
   GemmWsParams q;
   std::memset(&q, 0, sizeof(q));
   const uint64_t dimsA[2] = {(uint64_t)C, (uint64_t)rows};
@@ -366,14 +343,14 @@ int launch_gemm_ws(GemmParams& p, int mode, const void* A, long long rows, long 
   const uint32_t boxA[2] = {(uint32_t)WS_BK, (uint32_t)WS_BM};
   int rc = cached_tmap_bf16(&p.mapA, A, 2, dimsA, strA, boxA, 128);
   if (rc != PN_OK) return rc;
-  const uint64_t n_out = mode == 2 ? p.N / 2 : p.N;
-  if (mode == 0) {
+  const uint64_t n_out = mode == EPI_GEGLU ? p.N / 2 : p.N;
+  if (mode == EPI_F32) {
     rc = cached_tmap_f32_2d(&q.mapOut, p.out, n_out, rows, p.ldo, WS_BM);
   } else {
     const uint64_t dims[2] = {n_out, (uint64_t)rows};
     const uint64_t str[1] = {(uint64_t)p.ldo};
-    const uint32_t box[2] = {mode == 2 ? 16u : 32u, (uint32_t)WS_BM};
-    rc = cached_tmap_bf16(&q.mapOut, p.out, 2, dims, str, box, mode == 2 ? 32 : 64);
+    const uint32_t box[2] = {mode == EPI_GEGLU ? 16u : 32u, (uint32_t)WS_BM};
+    rc = cached_tmap_bf16(&q.mapOut, p.out, 2, dims, str, box, mode == EPI_GEGLU ? 32 : 64);
   }
   if (rc != PN_OK) return rc;
   if (p.residual != nullptr) {
@@ -392,7 +369,8 @@ int launch_gemm_ws(GemmParams& p, int mode, const void* A, long long rows, long 
   q.row_tiles = (int)((rows + WS_BM - 1) / WS_BM);
   q.groups = std::min(sm_count() / p.tiles_col, q.row_tiles);
   q.kc = C / WS_BK;
-  void (*kern)(GemmWsParams) = mode == 2 ? gemm_ws_kernel<2> : mode == 1 ? gemm_ws_kernel<1> : gemm_ws_kernel<0>;
+  void (*kern)(GemmWsParams) = mode == EPI_GEGLU ? gemm_ws_kernel<EPI_GEGLU>
+                              : mode == EPI_BF16 ? gemm_ws_kernel<EPI_BF16> : gemm_ws_kernel<EPI_F32>;
   rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), WS_SMEM);
   if (rc != PN_OK) return rc;
   kern<<<(unsigned)(q.groups * p.tiles_col), WS_THREADS, WS_SMEM, stream>>>(q);

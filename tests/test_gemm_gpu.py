@@ -3,32 +3,16 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from gemm_cases import _check, _rand
 from panacea_b200.ops import geglu_pack
 
 pytestmark = pytest.mark.gpu
-
-# the torch references below must be true fp32 (cuDNN/cuBLAS default to TF32 for conv/matmul on this GPU)
-torch.backends.cudnn.allow_tf32 = False
-torch.backends.cuda.matmul.allow_tf32 = False
 
 
 @pytest.fixture(scope="module")
 def ops():
     from panacea_b200.ops import NativeOps
     return NativeOps()
-
-
-def _rand(shape, seed, scale=1.0, dtype=torch.bfloat16):
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    return (torch.randn(shape, generator=g) * scale).to(dtype).cuda()
-
-
-def _check(got, ref, tol=2e-3, name=""):
-    got = got.float()
-    err = (got - ref).abs().max().item()
-    scale = ref.abs().max().item() + 1e-6
-    assert torch.isfinite(got).all(), f"{name}: non-finite output"
-    assert err <= tol * scale, f"{name}: max err {err:.4e} vs scale {scale:.3e}"
 
 
 @pytest.mark.parametrize("M,N,K", [(128, 160, 64), (256, 160, 128), (1000, 320, 320), (777, 128, 192),

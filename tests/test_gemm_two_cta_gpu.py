@@ -1,23 +1,26 @@
-"""GPU parity of the two-CTA-per-SM wgmma GEMM / implicit-conv kernel where its shallow shared-memory ring matters:
-reductions with fewer k-blocks than ring stages and long ones, every column tile width (BN = 160 / 128 / 64 / 32 with
-3 / 3 / 4 / 5 stages), every epilogue at the level-0 row count and at long reductions, 3x3 / 3x1 taps at the network's
-channel counts. Same torch fp32 references and tolerances as test_gemm_gpu.py."""
+"""GPU parity of the wgmma GEMM / implicit-conv kernels where the two-CTA-per-SM kernel's shallow shared-memory ring
+matters: reductions with fewer k-blocks than ring stages and long ones, every column tile width (BN = 160 / 128 / 64 / 32
+with 3 / 3 / 4 / 5 stages), every epilogue at the level-0 row count and at long reductions, 3x3 / 3x1 taps at the
+network's channel counts. Same torch fp32 references and tolerances as test_gemm_gpu.py. The level-0 epilogues at
+K = 320 are the shapes pn_gemm runs on the persistent kernel (gemm_ws.cu); every other case runs on gemm_tc_kernel, and
+the epilogue cases check which kernel ran."""
 import pytest
 import torch
 import torch.nn.functional as F
 
-from panacea_b200.ops import geglu_pack
-from test_gemm_gpu import _check, _rand, ops  # noqa: F401  (ops is the module-scoped NativeOps fixture)
+from gemm_cases import _check, _rand, _rand_dev, check_case, epilogue_case, kernels_of
+from test_gemm_gpu import ops  # noqa: F401  (the module-scoped NativeOps fixture)
 
 pytestmark = pytest.mark.gpu
 
 M0 = 172032          # level-0 rows of the benchmarked ε-evaluation: 16 frames x 32 x 336
 
 
-def _rand_dev(shape, seed, scale=1.0, dtype=torch.bfloat16):
-    """_rand drawn on the device: the level-0 operands have 10^8 elements."""
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    return (torch.randn(shape, generator=g, device="cuda") * scale).to(dtype)
+def _epilogue(ops, M, K, kind, kernel):
+    call, ref, tol = epilogue_case(ops, kind, M, K, seed=70)
+    got, ran = kernels_of(lambda: call(M))
+    assert ran and all(kernel in k for k in ran), ran
+    check_case(kind, got, ref, tol, name=f"{kind} {M}x{K}")
 
 
 @pytest.mark.parametrize("N", [320, 384, 64, 8])                   # BN = 160, 128, 64, 32
@@ -36,7 +39,7 @@ def test_reduction_length_every_tile_width(ops, K, N):
 @pytest.mark.parametrize("kind", ["f32_res_res2", "bf16_res_f32", "bf16_res_bf16", "ln_stats", "ln_fold", "geglu", "rowvec"])
 @pytest.mark.parametrize("K", [320, 1280])
 def test_level0_epilogues(ops, K, kind):
-    _epilogue_case(ops, M0, K, kind)
+    _epilogue(ops, M0, K, kind, "gemm_ws_kernel" if K == 320 else "gemm_tc_kernel")
 
 
 # 89 and 90 k-blocks: reductions as long as the level-1 3x3 convs, with a partial last k-block tap in the first case. A
@@ -44,70 +47,7 @@ def test_level0_epilogues(ops, K, kind):
 @pytest.mark.parametrize("kind", ["f32_res_res2", "bf16_res_f32", "bf16_res_bf16", "ln_stats", "geglu", "rowvec"])
 @pytest.mark.parametrize("K", [5696, 5760])
 def test_long_reduction_epilogues(ops, K, kind):
-    _epilogue_case(ops, 3000, K, kind)
-
-
-def _epilogue_case(ops, M, K, kind):
-    a = _rand_dev((M, K), 70)
-    if kind == "geglu":
-        N = 2560
-        w = _rand_dev((N, K), 71, K ** -0.5)
-        b = _rand_dev((N,), 72, dtype=torch.float32)
-        out = ops.gemm(a, geglu_pack(w), bias=geglu_pack(b), geglu=True, out_dtype=torch.bfloat16)
-        torch.cuda.synchronize()
-        y = a.float() @ w.float().t() + b
-        _check(out, y[:, :N // 2] * F.gelu(y[:, N // 2:]), tol=1e-2, name="geglu")
-        return
-    if kind in ("ln_stats", "ln_fold"):
-        from panacea_b200.engine import Engine
-        C = min(K, 1280)                # token-stream width: 320 at level 0, 1280 at level 2
-        wo = _rand_dev((C, K), 73, K ** -0.5)
-        y0 = _rand_dev((M, C), 74, 2.0) + 0.7
-        y, st = ops.gemm(a, wo, residual=y0, out_dtype=torch.bfloat16, ln_stats_out=True)
-        torch.cuda.synchronize()
-        yf = y.float()
-        if kind == "ln_stats":
-            _check(y, a.float() @ wo.float().t() + y0.float(), tol=1e-2, name="ln producer output")
-            torch.testing.assert_close(st[..., 0].sum(1), yf.sum(1), rtol=5e-3, atol=0.5)
-            torch.testing.assert_close(st[..., 1].sum(1), (yf * yf).sum(1), rtol=5e-3, atol=0.5)
-            return
-        gamma = _rand_dev((C,), 75, 0.2, dtype=torch.float32) + 1.0
-        beta = _rand_dev((C,), 76, 0.2, dtype=torch.float32)
-        wq = _rand_dev((960, C), 77, C ** -0.5, dtype=torch.float32)
-        wp, s, t = Engine._ln_fold_pack(wq, None, gamma, beta)
-        out = ops.gemm(y, wp, bias=t, out_dtype=torch.bfloat16, ln=(st, s, 1e-5))
-        torch.cuda.synchronize()
-        _check(out, F.layer_norm(yf, (C,), gamma, beta, 1e-5) @ wq.t(), tol=1.5e-2, name="LN fold -> linear")
-        return
-    N = 320
-    w = _rand_dev((N, K), 78, K ** -0.5)
-    bias = _rand_dev((N,), 79, dtype=torch.float32)
-    ref = a.float() @ w.float().t() + bias
-    if kind == "f32_res_res2":
-        r1 = _rand_dev((M, N), 80, dtype=torch.float32)
-        r2 = _rand_dev((M, N), 81, dtype=torch.float32)
-        out = ops.gemm(a, w, bias=bias, residual=r1, residual2=r2)
-        ref += r1 + r2
-        tol = 2e-3
-    elif kind == "bf16_res_f32":
-        r1 = _rand_dev((M, N), 82, dtype=torch.float32)
-        out = ops.gemm(a, w, bias=bias, residual=r1, out_dtype=torch.bfloat16)
-        ref += r1
-        tol = 1e-2
-    elif kind == "bf16_res_bf16":
-        r1 = _rand_dev((M, N), 83)
-        ref += r1.float()
-        out = ops.gemm(a, w, bias=bias, residual=r1, out=r1, out_dtype=torch.bfloat16)      # in place, like the token stream
-        tol = 1e-2
-    else:
-        G = 16
-        rv = _rand_dev((G, N), 84, dtype=torch.float32)
-        rpg = M // (2 * G)
-        out = ops.gemm(a, w, bias=bias, rowvec=rv, rows_per_group=rpg, n_groups=G)
-        ref += rv[(torch.arange(M, device="cuda") // rpg) % G]
-        tol = 2e-3
-    torch.cuda.synchronize()
-    _check(out, ref, tol=tol, name=kind)
+    _epilogue(ops, 3000, K, kind, "gemm_tc_kernel")
 
 
 @pytest.mark.parametrize("NB,H,W,C,N", [(16, 32, 336, 64, 320),      # UNet/ControlNet stem (input channels padded to 64)

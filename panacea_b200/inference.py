@@ -9,7 +9,8 @@ checkpoint provides `first_stage_model.*`. The OpenCLIP text tower is native too
 (`conditioner.embedders.0.model.*`) or from a stock open_clip file given as the embedder's `version`; prompts are
 tokenized with the CLIP BPE vocabulary at the embedder's `bpe_path` (else open_clip's bundled copy). Without weights the
 embedder is a deterministic stand-in. With the real modules importable, `--dataset module:Class` and the YAML targets
-swap them in. Overrides use the dotlist form, and a numeric component indexes a list:
+swap them in. `--clips K` generates scenes of K clips chained through their boundary frame (DESIGN.md section 11).
+Overrides use the dotlist form, and a numeric component indexes a list:
 
   torchrun --nproc-per-node 8 -m panacea_b200.inference --base configs.yaml --name run1 --inferdir out --gather
       --ckptpath panacea.ckpt model.params.conditioner_config.params.emb_models.0.params.bpe_path=bpe_simple_vocab_16e6.txt.gz
@@ -29,6 +30,7 @@ from torch.utils.data.distributed import DistributedSampler
 
 from . import dist_utils as D
 from . import frame_io as IO
+from .scene import scene_frame_number
 from .sgm.util import instantiate_from_config
 
 
@@ -36,13 +38,26 @@ class SyntheticBEVDataset(Dataset):
     """Batch contract of sgm/data/nuscenes_video/nuscenes_datasets_video.py:495-570 (`MyDataset.__getitem__`) with
     synthetic content: `jpg` target frames [T,3,H,6w] in [-1,1], `cond_img` the 19-channel BEV control maps [T,19,H,6w]
     in [0,1], `final_cond_zero` the image condition (zeros except the last — or first — frame, :559-566), `txt`,
-    `filenames` (per frame, per camera)."""
+    `filenames` (per frame, per camera).
 
-    def __init__(self, num_sequences=2, num_frames=8, image_hw=(256, 512), use_last_frame=True, seed=0):
+    Scene form (`clips` = K > 1, DESIGN.md section 11): an item is `{"clips": [clip_0, ..., clip_{K-1}]}`. Clip 0 is the
+    batch above; clips k > 0 carry only their layout, `cond_img`, `txt` and `filenames`, because their image condition
+    is a frame that clip k-1 generates. A boundary frame has the same file name in both clips that hold it."""
+
+    def __init__(self, num_sequences=2, num_frames=8, image_hw=(256, 512), use_last_frame=True, seed=0, clips=1):
         self.n, self.T, (self.h, self.w), self.use_last_frame, self.seed = num_sequences, num_frames, image_hw, use_last_frame, seed
+        if clips < 1:
+            raise ValueError(f"clips must be >= 1, got {clips}")
+        self.clips = clips
 
     def __len__(self):
         return self.n
+
+    def _names(self, idx, clip):
+        scene = f"n015-2018-07-24-11-22-45+0800__seq{idx:04d}"
+        stamp = lambda f: 1532402927 + 50 * scene_frame_number(clip, f, self.clips, self.T, self.use_last_frame)
+        return [[f"samples/{cam}/{scene}__{cam}__{stamp(f):d}.jpg" for cam in sorted(IO.VIEW_ID, key=IO.VIEW_ID.get)]
+                for f in range(self.T)]
 
     def __getitem__(self, idx):
         g = torch.Generator().manual_seed(self.seed * 100003 + idx)
@@ -51,11 +66,13 @@ class SyntheticBEVDataset(Dataset):
         cond = torch.zeros_like(target)
         k = -1 if self.use_last_frame else 0
         cond[k] = target[k]
-        scene = f"n015-2018-07-24-11-22-45+0800__seq{idx:04d}"
-        names = [[f"samples/{cam}/{scene}__{cam}__{1532402927 + 50 * f:d}.jpg" for cam in
-                  sorted(IO.VIEW_ID, key=IO.VIEW_ID.get)] for f in range(self.T)]
-        return {"jpg": target, "cond_img": torch.rand(self.T, 19, self.h, W, generator=g), "final_cond_zero": cond,
-                "txt": "a driving scene, six surround-view cameras", "filenames": names}
+        txt = "a driving scene, six surround-view cameras"
+        first = {"jpg": target, "cond_img": torch.rand(self.T, 19, self.h, W, generator=g), "final_cond_zero": cond,
+                 "txt": txt, "filenames": self._names(idx, 0)}
+        if self.clips == 1:
+            return first
+        return {"clips": [first] + [{"cond_img": torch.rand(self.T, 19, self.h, W, generator=g), "txt": txt,
+                                     "filenames": self._names(idx, c)} for c in range(1, self.clips)]}
 
 
 def load_config(paths, overrides=()):
@@ -131,7 +148,27 @@ def get_parser():
     p.add_argument("--image_hw", type=int, nargs=2, default=(256, 512), help="per-view image size of the synthetic dataset")
     p.add_argument("--gather", action="store_true", help="gather decoded frames on rank 0 and let rank 0 write them")
     p.add_argument("--randomize_zero_init", action="store_true", help="re-draw the reference's zero-initialised tails (no checkpoint)")
+    p.add_argument("--clips", type=_positive_int, default=1,
+                   help="clips per scene: each clip after the first is conditioned on a frame of the one before (DESIGN.md section 11)")
     return p
+
+
+def _positive_int(v) -> int:
+    n = int(v)
+    if n < 1:
+        raise argparse.ArgumentTypeError(f"must be >= 1, got {v}")
+    return n
+
+
+def make_dataset(opt, config):
+    """`--dataset module:Class` (constructed with `clips=` only for scenes, so a one-clip dataset needs no such keyword)
+    or the synthetic dataset; with --clips K > 1 every item is a scene `{"clips": [K clip batches]}`."""
+    if opt.dataset:
+        mod, cls = opt.dataset.split(":")
+        kw = {"clips": opt.clips} if opt.clips > 1 else {}
+        return getattr(importlib.import_module(mod), cls)(split=opt.split, use_last_frame=opt.use_last_frame, **kw)
+    T = config["model"]["params"]["network_config"]["params"].get("num_frames", 8)
+    return SyntheticBEVDataset(opt.num_sequences, T, tuple(opt.image_hw), opt.use_last_frame, seed=opt.seed, clips=opt.clips)
 
 
 def main(argv=None):
@@ -154,12 +191,7 @@ def main(argv=None):
     torch.manual_seed(seed)
     device = torch.device("cuda", local)
 
-    if opt.dataset:
-        mod, cls = opt.dataset.split(":")
-        dataset = getattr(importlib.import_module(mod), cls)(split=opt.split, use_last_frame=opt.use_last_frame)
-    else:
-        T = config["model"]["params"]["network_config"]["params"].get("num_frames", 8)
-        dataset = SyntheticBEVDataset(opt.num_sequences, T, tuple(opt.image_hw), opt.use_last_frame, seed=opt.seed)
+    dataset = make_dataset(opt, config)
     sampler = DistributedSampler(dataset, num_replicas=world, rank=rank, shuffle=False)
     loader = DataLoader(dataset, batch_size=opt.bs, sampler=sampler)
 
@@ -174,6 +206,13 @@ def main(argv=None):
     all_time, written = 0.0, []
     for idx, batch in enumerate(loader):
         start = time.time()
+        if opt.clips > 1:
+            written += _run_scene(model, batch, opt, inferdir, rank, world, device)
+            all_time += time.time() - start
+            if rank == 0:
+                print(f"idx {idx}: time per scene {time.time() - start:.2f}s ({opt.clips} clips), avg {all_time / (idx + 1):.2f}s",
+                      flush=True)
+            continue
         for key in batch:
             if key not in ("txt", "filenames"):
                 batch[key] = batch[key].to(device)
@@ -199,6 +238,25 @@ def main(argv=None):
         dist.barrier()
         dist.destroy_process_group()
     return written
+
+
+def _run_scene(model, item, opt, inferdir, rank, world, device) -> list[str]:
+    """One scene of `opt.clips` clips (`DiffusionEngine3D.sample_scene`), written as one chronological sequence per
+    camera plus one PNG strip and one GIF; `--gather` gathers one scene per rank on rank 0."""
+    clips = item["clips"]
+    if len(clips) != opt.clips:
+        raise ValueError(f"--clips {opt.clips}, but the dataset item holds {len(clips)} clips")
+    with torch.no_grad():
+        out = model.sample_scene(clips, use_last_frame=opt.use_last_frame)
+    frames, names = out["samples"], out["filenames"]
+    if opt.gather and world > 1:
+        gathered = D.gather_on_rank0(frames.to(device).contiguous())
+        all_names = [None] * world
+        dist.all_gather_object(all_names, names)
+        if rank != 0:
+            return []
+        return [w for r in range(world) for w in IO.logs_scene(gathered[r], inferdir, all_names[r])]
+    return IO.logs_scene(frames, inferdir, names)
 
 
 if __name__ == "__main__":

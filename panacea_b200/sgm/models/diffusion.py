@@ -90,18 +90,26 @@ class DiffusionEngine3D(nn.Module):
         """diffusion.py:300-377 for the SD-2.1 branch the config takes (unconditional prompt = ""), without the text/cond
         renderings (log_conditionings draws strings with PIL fonts — not part of the data path)."""
         log = {}
-        x = self.get_input(batch)
         if "cond_img" in batch:
             log["cond_img"] = batch["cond_img"].reshape(-1, *batch["cond_img"].shape[2:]).contiguous()
         batch_uc = dict(batch)
         batch_uc["txt"] = ["" for _ in batch["txt"]]                                # diffusion.py:329-331
         c, uc = self.conditioner.get_unconditional_conditioning(batch, batch_uc=batch_uc, force_uc_zero_embeddings=[])
-        N = min(x.shape[0], N)
-        x = x.to(self.device)[:N]
-        x = x.reshape(-1, *x.shape[2:]).contiguous()                                 # "b t c h w -> (b t) c h w"
-        log["inputs"] = x
-        z = self.encode_first_stage(x)
-        log["reconstructions"] = self.decode_first_stage(z)
+        if self.input_key in batch:
+            x = self.get_input(batch)
+            N = min(x.shape[0], N)
+            x = x.to(self.device)[:N]
+            x = x.reshape(-1, *x.shape[2:]).contiguous()                             # "b t c h w -> (b t) c h w"
+            log["inputs"] = x
+            z = self.encode_first_stage(x)
+            log["reconstructions"] = self.decode_first_stage(z)
+            latent_shape = z.shape[1:]
+        else:
+            # no ground truth (the clips k > 0 of a scene): the latent shape comes from the image condition
+            if "concat" not in c:
+                raise KeyError(f"batch has no {self.input_key!r} and the conditioner produces no 'concat' to take the latent shape from")
+            N = min(c["concat"].shape[0] // self.num_frames, N)
+            latent_shape = c["concat"].shape[1:]
         if "cond_feat" in c:
             log["control"] = c["cond_feat"] * 2.0 - 1.0
         for k in c:                                                                  # diffusion.py:356-364
@@ -113,7 +121,55 @@ class DiffusionEngine3D(nn.Module):
                 else:
                     c[k], uc[k] = (y[k][:N].to(self.device) for y in (c, uc))
         if sample:
-            samples = self.sample(c, shape=z.shape[1:], uc=uc, batch_size=N * self.num_frames)
+            samples = self.sample(c, shape=latent_shape, uc=uc, batch_size=N * self.num_frames)
             log["samples"] = self.decode_first_stage(samples)
             log["sample_latents"] = samples
         return log
+
+    def _image_condition_key(self) -> str:
+        keys = [e.input_key for e in self.conditioner.embedders if isinstance(e, VAEEmbedder)]
+        if len(keys) != 1:
+            raise ValueError(f"a scene needs exactly one VAEEmbedder image condition in the conditioner, found {len(keys)}")
+        return keys[0]
+
+    @torch.no_grad()
+    def sample_scene(self, batches, use_last_frame=True, **kwargs):
+        """A scene of K = len(batches) clips chained through their boundary frame (panacea_b200/scene.py).
+
+        `batches[k]` is clip k's layout batch as `MyDataset.__getitem__` + the DataLoader give it (one sequence):
+        `cond_img`, `txt`, `filenames`; clip 0 also carries the ground truth and its real image condition. Tensors may
+        stay on the host: each clip's are moved to the device when that clip runs. Clip k > 0 is
+        conditioned on the frame of clip k-1 at index T-1-a (a = T-1 with `use_last_frame`, else 0), quantised like the
+        writers and read back like the dataset, in a `final_cond_zero` that is zero elsewhere; it goes through the
+        conditioner and the VAE embedder unchanged. Each clip is one `log_images` call, in clip order, so the CPU
+        generator is drawn as K successive calls draw it, and K = 1 is exactly `log_images`. The wrapper replays the
+        one CUDA graph of clip 0 (the conditioning is re-prepared into the same buffers). A clip's decoded frames move
+        to the host before the next clip starts, so the device peak of a scene is that of one clip.
+
+        Returns a dict (all tensors on the host): "samples" the scene [K(T-1)+1, 3, H, W] in chronological order,
+        "sample_latents" the K per-clip latents [T, 4, h, w], "handoff_frames" the K-1 dequantised frames [3, H, W]
+        that conditioned clips 1..K-1, "clip_samples" the K decoded clips [T, 3, H, W], and "filenames" in scene order
+        when the batches carry them."""
+        from ... import scene as S
+        T = self.num_frames
+        key = self._image_condition_key() if len(batches) > 1 else None
+        clips, latents, handoffs = [], [], []
+        for k, batch in enumerate(batches):
+            batch = {n: v.to(self.device) if isinstance(v, torch.Tensor) else v for n, v in batch.items()}   # one clip at a time
+            if k > 0:
+                cond = S.condition_from_frame(handoffs[-1], T, use_last_frame)
+                batch = {n: v for n, v in batch.items() if n != self.input_key}
+                batch[key] = cond.unsqueeze(0).to(self.device)
+            log = self.log_images(batch, **kwargs)
+            if log["samples"].shape[0] != T:
+                raise ValueError(f"a scene clip is one sequence of {T} frames; clip {k} decoded {log['samples'].shape[0]}")
+            clips.append(log["samples"].cpu())
+            latents.append(log["sample_latents"].cpu())
+            del log                                                         # the clip's device tensors go before the next clip
+            if k + 1 < len(batches):
+                handoffs.append(S.quantize_frame(clips[-1][S.handoff_index(T, use_last_frame)]))
+        out = {"samples": S.scene_order(clips, use_last_frame), "sample_latents": latents, "handoff_frames": handoffs,
+               "clip_samples": clips}
+        if all("filenames" in b for b in batches):
+            out["filenames"] = S.scene_order([b["filenames"] for b in batches], use_last_frame)
+        return out

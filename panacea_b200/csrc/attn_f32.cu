@@ -113,7 +113,7 @@ __global__ void __launch_bounds__(AF_QTILE) attn_f32_view_kernel(const AfParams 
     for (int d = 0; d < D; d += 8) {
       const float v8[8] = {o[d] * inv, o[d + 1] * inv, o[d + 2] * inv, o[d + 3] * inv,
                            o[d + 4] * inv, o[d + 5] * inv, o[d + 6] * inv, o[d + 7] * inv};
-      store_op8<OP>(p.out, (size_t)qtok, p.out_C, head * D + d, v8);
+      store_op<OP>(p.out, (size_t)qtok, p.out_C, head * D + d, v8);
     }
   }
 }
@@ -170,7 +170,7 @@ __global__ void __launch_bounds__(128) attn_f32_temporal_kernel(const float* __r
   for (int d = 0; d < D; d += 8) {
     const float v8[8] = {o[d] * inv, o[d + 1] * inv, o[d + 2] * inv, o[d + 3] * inv,
                          o[d + 4] * inv, o[d + 5] * inv, o[d + 6] * inv, o[d + 7] * inv};
-    store_op8<OP>(out, (size_t)qtok, heads * D, head * D + d, v8);
+    store_op<OP>(out, (size_t)qtok, heads * D, head * D + d, v8);
   }
 }
 
@@ -228,12 +228,14 @@ __global__ void __launch_bounds__(128) attn_f32_causal_kernel(const float* __res
   for (int d = 0; d < D; d += 8) {
     const float v8[8] = {o[d] * inv, o[d + 1] * inv, o[d + 2] * inv, o[d + 3] * inv,
                          o[d + 4] * inv, o[d + 5] * inv, o[d + 6] * inv, o[d + 7] * inv};
-    store_op8<OP>(out, (size_t)(row0 + qi), heads * D, head * D + d, v8);
+    store_op<OP>(out, (size_t)(row0 + qi), heads * D, head * D + d, v8);
   }
 }
 
 // The parity-mode launchers behind pn_attention / pn_attention_temporal / pn_attention_causal (declared in common.cuh):
-// those entry points call them for operand_mode PN_OPERAND_SPLIT3 / PN_OPERAND_F32.
+// those entry points check operand_mode and call them for the two modes below.
+using F32Modes = OperandModes<PN_OPERAND_SPLIT3, PN_OPERAND_F32>;
+
 int attention_causal_f32(const float* q, const float* k, const float* v, void* out, int64_t batch, int64_t L, int32_t heads,
                          int32_t head_dim, int64_t ld, int64_t out_ld, float scale, int operand_mode, void* stream_v) {
   PN_REQUIRE(q && k && v && out, "pn_attention_causal: null pointer");
@@ -245,7 +247,7 @@ int attention_causal_f32(const float* q, const float* k, const float* v, void* o
   const long long blocks = (total + 127) / 128;
   PN_REQUIRE(blocks < (1ll << 31), "pn_attention_causal: grid too large");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  PN_DISPATCH_OP(operand_mode, attn_f32_causal_kernel<OP><<<(unsigned)blocks, 128, 0, st>>>(q, k, v, out, (int)batch, (int)L, heads, ld,
+  PN_DISPATCH_OP(F32Modes, operand_mode, attn_f32_causal_kernel<OP><<<(unsigned)blocks, 128, 0, st>>>(q, k, v, out, (int)batch, (int)L, heads, ld,
                                                                                          scale * 1.4426950408889634f));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
@@ -281,8 +283,8 @@ int attention_f32(const pn_attn_args* a, int operand_mode, void* stream_v) {
   const long long blocks = tiles * a->heads * a->V * a->F;
   PN_REQUIRE(blocks > 0 && blocks < (1ll << 31), "pn_attention: grid too large");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  if (a->head_dim == 64) PN_DISPATCH_OP(operand_mode, attn_f32_view_kernel<64, OP><<<(unsigned)blocks, AF_QTILE, 0, st>>>(p));
-  else PN_DISPATCH_OP(operand_mode, attn_f32_view_kernel<80, OP><<<(unsigned)blocks, AF_QTILE, 0, st>>>(p));
+  if (a->head_dim == 64) PN_DISPATCH_OP(F32Modes, operand_mode, attn_f32_view_kernel<64, OP><<<(unsigned)blocks, AF_QTILE, 0, st>>>(p));
+  else PN_DISPATCH_OP(F32Modes, operand_mode, attn_f32_view_kernel<80, OP><<<(unsigned)blocks, AF_QTILE, 0, st>>>(p));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
@@ -301,9 +303,9 @@ int attention_temporal_f32(const float* q, const float* k, const float* v, void*
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   const float sl2 = scale * 1.4426950408889634f;
   if (head_dim == 64)
-    PN_DISPATCH_OP(operand_mode, attn_f32_temporal_kernel<64, OP><<<(unsigned)blocks, 128, 0, st>>>(q, k, v, out, (int)batch, (int)T, (int)pixels, heads, ld, sl2));
+    PN_DISPATCH_OP(F32Modes, operand_mode, attn_f32_temporal_kernel<64, OP><<<(unsigned)blocks, 128, 0, st>>>(q, k, v, out, (int)batch, (int)T, (int)pixels, heads, ld, sl2));
   else
-    PN_DISPATCH_OP(operand_mode, attn_f32_temporal_kernel<80, OP><<<(unsigned)blocks, 128, 0, st>>>(q, k, v, out, (int)batch, (int)T, (int)pixels, heads, ld, sl2));
+    PN_DISPATCH_OP(F32Modes, operand_mode, attn_f32_temporal_kernel<80, OP><<<(unsigned)blocks, 128, 0, st>>>(q, k, v, out, (int)batch, (int)T, (int)pixels, heads, ld, sl2));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }

@@ -22,6 +22,7 @@
 // O = P V a second wgmma of N = 16 per key step into output channels 64..79.
 #include "common.cuh"
 #include "ptx.cuh"
+#include "operand.cuh"
 #include "../../include/panacea_b200.h"
 
 namespace pn {
@@ -252,8 +253,8 @@ __global__ void __launch_bounds__(FA_THREADS, 1) attn_fa_kernel(const __grid_con
 using namespace pn;
 
 extern "C" int pn_attention(const pn_attn_args* a, int operand_mode, void* stream_v) {
-  if (operand_mode == PN_OPERAND_SPLIT3 || operand_mode == PN_OPERAND_F32) return attention_f32(a, operand_mode, stream_v);
-  PN_REQUIRE(operand_mode == PN_OPERAND_BF16, "pn_attention: operand_mode %d unsupported (0, 1 or 2)", operand_mode);
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_attention", PN_OPERAND_BF16, PN_OPERAND_SPLIT3, PN_OPERAND_F32);
+  if (operand_mode != PN_OPERAND_BF16) return attention_f32(a, operand_mode, stream_v);
   if (a == nullptr) return fail(PN_ERR_INVALID, "pn_attention: null args");
   PN_REQUIRE(a->q && a->k && a->v && a->out, "pn_attention: null tensor pointer");
   PN_REQUIRE(a->head_dim == 64 || a->head_dim == 80, "pn_attention: head_dim %d unsupported (64 or 80)", a->head_dim);

@@ -9,6 +9,7 @@
 // "(b t)(h w) c -> (b h w) t c" rearrangement of the reference is just this indexing — nothing is copied.
 #include "common.cuh"
 #include "ptx.cuh"
+#include "operand.cuh"
 #include "../../include/panacea_b200.h"
 
 namespace pn {
@@ -271,11 +272,11 @@ using namespace pn;
 extern "C" int pn_attention_causal(const void* q, const void* k, const void* v, void* out, int64_t batch, int64_t L,
                                    int32_t heads, int32_t head_dim, int64_t ld, int64_t out_ld, float scale, int operand_mode,
                                    void* stream_v) {
-  if (operand_mode == PN_OPERAND_SPLIT3 || operand_mode == PN_OPERAND_F32)
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_attention_causal", PN_OPERAND_BF16, PN_OPERAND_SPLIT3, PN_OPERAND_F32);
+  if (operand_mode != PN_OPERAND_BF16)
     return attention_causal_f32(reinterpret_cast<const float*>(q), reinterpret_cast<const float*>(k),
                                 reinterpret_cast<const float*>(v), out, batch, L, heads, head_dim, ld, out_ld, scale, operand_mode,
                                 stream_v);
-  PN_REQUIRE(operand_mode == PN_OPERAND_BF16, "pn_attention_causal: operand_mode %d unsupported (0, 1 or 2)", operand_mode);
   PN_REQUIRE(q && k && v && out, "pn_attention_causal: null pointer");
   PN_REQUIRE(head_dim == CA_D, "pn_attention_causal: head_dim %d unsupported (64)", head_dim);
   PN_REQUIRE(L >= 1 && L <= CA_MAXL, "pn_attention_causal: L=%lld out of range 1..128", (long long)L);
@@ -300,11 +301,11 @@ extern "C" int pn_attention_causal(const void* q, const void* k, const void* v, 
 extern "C" int pn_attention_temporal(const void* q, const void* k, const void* v, void* out, int64_t batch, int64_t T,
                                      int64_t pixels, int32_t heads, int32_t head_dim, int64_t ld, int64_t out_ld,
                                      float scale, int operand_mode, void* stream_v) {
-  if (operand_mode == PN_OPERAND_SPLIT3 || operand_mode == PN_OPERAND_F32)
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_attention_temporal", PN_OPERAND_BF16, PN_OPERAND_SPLIT3, PN_OPERAND_F32);
+  if (operand_mode != PN_OPERAND_BF16)
     return attention_temporal_f32(reinterpret_cast<const float*>(q), reinterpret_cast<const float*>(k),
                                   reinterpret_cast<const float*>(v), out, batch, T, pixels, heads, head_dim, ld, out_ld, scale,
                                   operand_mode, stream_v);
-  PN_REQUIRE(operand_mode == PN_OPERAND_BF16, "pn_attention_temporal: operand_mode %d unsupported (0, 1 or 2)", operand_mode);
   PN_REQUIRE(q && k && v && out, "pn_attention_temporal: null pointer");
   PN_REQUIRE(head_dim == 64 || head_dim == 80, "pn_attention_temporal: head_dim %d unsupported (64 or 80)", head_dim);
   PN_REQUIRE(T >= 1 && T <= TA_MAXT, "pn_attention_temporal: T=%lld out of range 1..16", (long long)T);

@@ -42,7 +42,7 @@ __global__ void upsample2x_kernel(const float* __restrict__ x, void* __restrict_
     const float4 a = *reinterpret_cast<const float4*>(src);
     const float4 b = *reinterpret_cast<const float4*>(src + 4);
     const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-    store_op8<OP>(y, ((size_t)f * 2 * H + oy) * 2 * W + ox, C, c8 * 8, v);
+    store_op<OP>(y, ((size_t)f * 2 * H + oy) * 2 * W + ox, C, c8 * 8, v);
   }
 }
 
@@ -87,7 +87,7 @@ __global__ void cast_operand_kernel(const float* __restrict__ x, void* __restric
   for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n4; e += (size_t)gridDim.x * blockDim.x) {
     const float4 a = reinterpret_cast<const float4*>(x)[e];
     const float v[4] = {a.x, a.y, a.z, a.w};
-    store_op4<OP>(y, e / c4n, C, (int)(e % c4n) * 4, v);
+    store_op<OP>(y, e / c4n, C, (int)(e % c4n) * 4, v);
   }
 }
 
@@ -108,7 +108,7 @@ __global__ void geglu_operand_kernel(const float* __restrict__ in, void* __restr
     float o[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) o[i] = vv[i] * (0.5f * gg[i] * (1.0f + erff(gg[i] * 0.70710678118654752f)));
-    store_op4<OP>(y, row, inner, col, o);
+    store_op<OP>(y, row, inner, col, o);
   }
 }
 
@@ -123,7 +123,7 @@ __global__ void gelu_operand_kernel(const float* __restrict__ x, void* __restric
     float o[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) o[i] = 0.5f * in[i] * (1.0f + erff(in[i] * 0.70710678118654752f));
-    store_op4<OP>(y, e / c4n, C, (int)(e % c4n) * 4, o);
+    store_op<OP>(y, e / c4n, C, (int)(e % c4n) * 4, o);
   }
 }
 
@@ -255,7 +255,7 @@ __global__ void im2col_s2_kernel(const float* __restrict__ x, void* __restrict__
       const float4 b = *reinterpret_cast<const float4*>(src + 4);
       v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
     }
-    store_op8<OP>(out, (((size_t)f * Ho + oy) * Wo + ox) * 9 + tap, C, c8 * 8, v);
+    store_op<OP>(out, (((size_t)f * Ho + oy) * Wo + ox) * 9 + tap, C, c8 * 8, v);
   }
 }
 
@@ -269,8 +269,8 @@ __global__ void scale_dup_kernel(const float* __restrict__ x, float* __restrict_
 // ---------------------------------------------------------------- row softmax, fp32 scores -> GEMM operand
 // The single-head, C-wide attention of the VAE mid block (reference model.py:374-414: SDPA over all h*w tokens with
 // head_dim = C = 512) is run as GEMMs (S = q k^T, O = P v) around this kernel: out[r, :] = softmax(scale * in[r, :]),
-// stored as the A operand of the O GEMM: bf16 [rows, N] (OP = PN_OP_BF16) or split3 [rows, 3N] = [hi | lo | hi]
-// (OP = PN_OP_SPLIT3, parity mode). ld_out counts bf16 elements. One CTA per row; the row's exponentials are kept in
+// stored as the A operand of the O GEMM: bf16 [rows, N] (OP = PN_OPERAND_BF16) or split3 [rows, 3N] = [hi | lo | hi]
+// (OP = PN_OPERAND_SPLIT3, parity mode). ld_out counts bf16 elements. One CTA per row; the row's exponentials are kept in
 // shared memory between the sum and the normalised store.
 template <int OP>
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ in, __nv_bfloat16* __restrict__ out, int N,
@@ -314,7 +314,7 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
   for (int i = threadIdx.x * 4; i < N; i += 1024) {
     const float4 v = *reinterpret_cast<float4*>(sm_row + i);
     const float o[4] = {v.x * inv, v.y * inv, v.z * inv, v.w * inv};
-    store_op4<OP>(dst, 0, N, i, o);       // row 0 of a "matrix" starting at this row: split3 thirds at +N, +2N
+    store_op<OP>(dst, 0, N, i, o);       // row 0 of a "matrix" starting at this row: split3 thirds at +N, +2N
   }
 }
 
@@ -357,10 +357,10 @@ extern "C" int pn_transpose_f32(const float* in, float* out, int64_t batch, int6
 
 extern "C" int pn_upsample2x(const float* x, void* y, int64_t frames, int64_t H, int64_t W, int64_t C, int operand_mode,
                              void* stream_v) {
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_upsample2x", PN_OPERAND_BF16, PN_OPERAND_SPLIT3, PN_OPERAND_F32);
   PN_REQUIRE(x && y && frames > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "pn_upsample2x: bad arguments");
-  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_upsample2x: operand_mode %d", operand_mode);
   const size_t total = (size_t)frames * 4 * H * W * (C / 8);
-  PN_DISPATCH_OP(operand_mode, upsample2x_kernel<OP><<<stride_grid(total), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
+  PN_DISPATCH_OP(Modes, operand_mode, upsample2x_kernel<OP><<<stride_grid(total), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
       x, y, (int)frames, (int)H, (int)W, (int)C));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
@@ -383,34 +383,30 @@ extern "C" int pn_add_inplace(float* x, const float* y, int64_t n, void* stream_
 }
 
 extern "C" int pn_cast_operand(const float* x, void* y, int64_t rows, int64_t C, int operand_mode, void* stream_v) {
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_cast_operand", PN_OPERAND_BF16, PN_OPERAND_SPLIT3, PN_OPERAND_SPLIT3_B);
   PN_REQUIRE(x && y && rows > 0 && C > 0 && C % 4 == 0, "pn_cast_operand: bad arguments");
-  PN_REQUIRE(operand_mode == PN_OP_BF16 || operand_mode == PN_OP_SPLIT3 || operand_mode == PN_OP_SPLIT3_B,
-             "pn_cast_operand: operand_mode %d", operand_mode);
   const size_t n4 = (size_t)rows * (size_t)(C / 4);
-  if (operand_mode == PN_OP_SPLIT3_B)
-    cast_operand_kernel<PN_OP_SPLIT3_B><<<stride_grid(n4), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(x, y, (size_t)rows, (int)C);
-  else
-    PN_DISPATCH_OP(operand_mode, cast_operand_kernel<OP><<<stride_grid(n4), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
-        x, y, (size_t)rows, (int)C));
+  PN_DISPATCH_OP(Modes, operand_mode, cast_operand_kernel<OP><<<stride_grid(n4), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
+      x, y, (size_t)rows, (int)C));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
 
 extern "C" int pn_geglu_operand(const float* in, void* y, int64_t rows, int64_t inner, int operand_mode, void* stream_v) {
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_geglu_operand", PN_OPERAND_BF16, PN_OPERAND_SPLIT3, PN_OPERAND_F32);
   PN_REQUIRE(in && y && rows > 0 && inner > 0 && inner % 16 == 0, "pn_geglu_operand: bad arguments");
-  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_geglu_operand: operand_mode %d", operand_mode);
   const size_t n4 = (size_t)rows * (size_t)(inner / 4);
-  PN_DISPATCH_OP(operand_mode, geglu_operand_kernel<OP><<<stride_grid(n4), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
+  PN_DISPATCH_OP(Modes, operand_mode, geglu_operand_kernel<OP><<<stride_grid(n4), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
       in, y, (size_t)rows, (int)inner));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }
 
 extern "C" int pn_gelu_operand(const float* x, void* y, int64_t rows, int64_t C, int operand_mode, void* stream_v) {
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_gelu_operand", PN_OPERAND_BF16, PN_OPERAND_SPLIT3, PN_OPERAND_F32);
   PN_REQUIRE(x && y && rows > 0 && C > 0 && C % 4 == 0, "pn_gelu_operand: bad arguments");
-  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_gelu_operand: operand_mode %d", operand_mode);
   const size_t n4 = (size_t)rows * (size_t)(C / 4);
-  PN_DISPATCH_OP(operand_mode, gelu_operand_kernel<OP><<<stride_grid(n4), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
+  PN_DISPATCH_OP(Modes, operand_mode, gelu_operand_kernel<OP><<<stride_grid(n4), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
       x, y, (size_t)rows, (int)C));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
@@ -461,13 +457,13 @@ extern "C" int pn_linear_small(const float* x, const void* W_any, int w_is_f32, 
 
 extern "C" int pn_im2col3x3_s2(const float* x, void* out, int64_t frames, int64_t H, int64_t W, int64_t C, int pad,
                                int operand_mode, void* stream_v) {
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_im2col3x3_s2", PN_OPERAND_BF16, PN_OPERAND_SPLIT3);
   PN_REQUIRE(x && out && frames > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "pn_im2col3x3_s2: bad arguments");
-  PN_REQUIRE(operand_mode == PN_OP_BF16 || operand_mode == PN_OP_SPLIT3, "pn_im2col3x3_s2: operand_mode %d", operand_mode);
   PN_REQUIRE(pad == 0 || pad == 1, "pn_im2col3x3_s2: pad must be 1 (symmetric) or 0 (zero row/column appended at the far edges)");
   // pad 1: Conv2d(k3, s2, padding=1); pad 0: F.pad(x, (0,1,0,1)) + Conv2d(k3, s2, padding=0) (the VAE encoder's Downsample)
   const int Ho = (int)((H + 2 * pad + (1 - pad) - 3) / 2 + 1), Wo = (int)((W + 2 * pad + (1 - pad) - 3) / 2 + 1);
   const size_t total = (size_t)frames * Ho * Wo * 9 * (C / 8);
-  PN_DISPATCH_OP(operand_mode, im2col_s2_kernel<OP><<<stride_grid(total), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
+  PN_DISPATCH_OP(Modes, operand_mode, im2col_s2_kernel<OP><<<stride_grid(total), 256, 0, reinterpret_cast<cudaStream_t>(stream_v)>>>(
       x, out, (int)frames, (int)H, (int)W, (int)C, Ho, Wo, pad));
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
@@ -494,19 +490,19 @@ extern "C" int pn_fingerprint(const void* x, int64_t nbytes, uint64_t* out2, voi
 
 extern "C" int pn_softmax_rows_operand(const float* in, void* out, int64_t rows, int64_t N, int64_t ld_in, int64_t ld_out, float scale,
                                        int operand_mode, void* stream_v) {
-  PN_REQUIRE(operand_mode == PN_OP_BF16 || operand_mode == PN_OP_SPLIT3, "pn_softmax_rows_operand: operand_mode %d", operand_mode);
-  const int64_t width = operand_mode == PN_OP_SPLIT3 ? 3 * N : N;
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_softmax_rows_operand", PN_OPERAND_BF16, PN_OPERAND_SPLIT3);
+  const int64_t width = operand_mode == PN_OPERAND_SPLIT3 ? 3 * N : N;
   PN_REQUIRE(in && out && rows > 0 && N > 0 && N % 4 == 0 && ld_in >= N && ld_out >= width && ld_in % 4 == 0 && ld_out % 4 == 0,
              "pn_softmax_rows_operand: bad arguments");
   PN_REQUIRE(N * 4 <= 200 * 1024, "pn_softmax_rows_operand: N=%lld exceeds the shared-memory row buffer", (long long)N);
   PN_REQUIRE(rows < (1ll << 31), "pn_softmax_rows_operand: too many rows");
   const size_t smem = (size_t)N * sizeof(float);
-  void (*kern)(const float*, __nv_bfloat16*, int, long long, long long, float) =
-      operand_mode == PN_OP_SPLIT3 ? softmax_rows_kernel<PN_OP_SPLIT3> : softmax_rows_kernel<PN_OP_BF16>;
-  const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem);
+  int rc = PN_OK;
+  PN_DISPATCH_OP(Modes, operand_mode,
+                 rc = ensure_dyn_smem(reinterpret_cast<const void*>(&softmax_rows_kernel<OP>), smem);
+                 if (rc == PN_OK) softmax_rows_kernel<OP><<<(unsigned)rows, 256, smem, reinterpret_cast<cudaStream_t>(stream_v)>>>(
+                     in, reinterpret_cast<__nv_bfloat16*>(out), (int)N, ld_in, ld_out, scale * 1.4426950408889634f));
   if (rc != PN_OK) return rc;
-  kern<<<(unsigned)rows, 256, smem, reinterpret_cast<cudaStream_t>(stream_v)>>>(in, reinterpret_cast<__nv_bfloat16*>(out), (int)N, ld_in,
-                                                                               ld_out, scale * 1.4426950408889634f);
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
 }

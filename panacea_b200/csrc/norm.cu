@@ -161,13 +161,13 @@ gn_fused_kernel(const float* __restrict__ x, const float* __restrict__ gamma, co
         auto emit = [&](size_t off, const float4& a, const float4& b) {
           float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
           const size_t row = row0 + off / (size_t)C;
-          if (raw) store_op8<OP>(raw, row, C, c8 * 8, v);
+          if (raw) store_op<OP>(raw, row, C, c8 * 8, v);
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const float t = v[j] * sc[j] + sh[j];
             v[j] = act_silu ? silu(t) : t;
           }
-          store_op8<OP>(y, row, C, c8 * 8, v);
+          store_op<OP>(y, row, C, c8 * 8, v);
         };
         int p = p0 + pl;
         for (; p + 3 * PL < p1; p += 4 * PL) {      // four pixels in flight per thread
@@ -241,7 +241,8 @@ __global__ void __launch_bounds__(512) gn_pixel_kernel(const float* __restrict__
     float a0 = (v[2 * j] - mean) * rstd * gm.x + bt.x;
     float a1 = (v[2 * j + 1] - mean) * rstd * gm.y + bt.y;
     if (act_silu) { a0 = silu(a0); a1 = silu(a1); }
-    store_op2<OP>(y, row, C, g * CPG + 2 * j, a0, a1);
+    const float o[2] = {a0, a1};
+    store_op<OP>(y, row, C, g * CPG + 2 * j, o);
   }
 }
 
@@ -302,7 +303,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const TIn* __restrict__ 
       const float o2 = (v[i].z - mean) * rstd * g.z + bb.z;
       const float o3 = (v[i].w - mean) * rstd * g.w + bb.w;
       const float o[4] = {o0, o1, o2, o3};
-      store_op4<OP>(y, (size_t)row, C, j * 4, o);
+      store_op<OP>(y, (size_t)row, C, j * 4, o);
     }
   }
 }
@@ -430,12 +431,12 @@ static int gn_launch(bool cooperative, int grid, size_t smem, cudaStream_t st, c
 extern "C" int pn_groupnorm_silu(const float* x, const float* gamma, const float* beta, void* y, void* raw,
                                  float* workspace, int64_t frames, int64_t pixels, int64_t channels, float eps,
                                  int act_silu, int operand_mode, void* stream_v) {
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_groupnorm_silu", PN_OPERAND_BF16, PN_OPERAND_SPLIT3, PN_OPERAND_F32);
   PN_REQUIRE(x && gamma && beta && y && workspace, "pn_groupnorm_silu: null pointer");
   PN_REQUIRE(channels % 32 == 0 && channels % 8 == 0 && channels <= 8192, "pn_groupnorm_silu: C=%lld unsupported",
              (long long)channels);
   PN_REQUIRE(frames > 0 && pixels > 0, "pn_groupnorm_silu: empty input");
   PN_REQUIRE(frames <= GN_MAX_FRAMES, "pn_groupnorm_silu: more than %d frames", GN_MAX_FRAMES);
-  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_groupnorm_silu: operand_mode %d", operand_mode);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   const int P = (int)pixels, C = (int)channels, F = (int)frames;
   int wave, cpf;
@@ -453,27 +454,27 @@ extern "C" int pn_groupnorm_silu(const float* x, const float* gamma, const float
   static const bool force_two_phase = [] { const char* e = std::getenv("PN_GN_TWO_PHASE"); return e && std::atoi(e) != 0; }();
   if (force_two_phase) {
     int rc = PN_OK;
-    PN_DISPATCH_OP(operand_mode, rc = gn_launch<OP, 1>(false, grid, smem, st, x, gamma, beta, y, raw, partial, arrive, P, C, F, wave,
-                                                        cpf, eps, act_silu));
+    PN_DISPATCH_OP(Modes, operand_mode, rc = gn_launch<OP, 1>(false, grid, smem, st, x, gamma, beta, y, raw, partial, arrive, P, C, F,
+                                                               wave, cpf, eps, act_silu));
     if (rc != PN_OK) return rc;
-    PN_DISPATCH_OP(operand_mode, rc = gn_launch<OP, 2>(false, grid, smem, st, x, gamma, beta, y, raw, partial, arrive, P, C, F, wave,
-                                                        cpf, eps, act_silu));
+    PN_DISPATCH_OP(Modes, operand_mode, rc = gn_launch<OP, 2>(false, grid, smem, st, x, gamma, beta, y, raw, partial, arrive, P, C, F,
+                                                               wave, cpf, eps, act_silu));
     return rc;
   }
   PN_CHECK_CUDA(cudaMemsetAsync(arrive, 0, sizeof(unsigned int) * (size_t)F, st));
   int rc = PN_OK;
-  PN_DISPATCH_OP(operand_mode, rc = gn_launch<OP, 0>(true, grid, smem, st, x, gamma, beta, y, raw, partial, arrive, P, C, F, wave,
-                                                      cpf, eps, act_silu));
+  PN_DISPATCH_OP(Modes, operand_mode, rc = gn_launch<OP, 0>(true, grid, smem, st, x, gamma, beta, y, raw, partial, arrive, P, C, F,
+                                                             wave, cpf, eps, act_silu));
   return rc;
 }
 
 extern "C" int pn_groupnorm_pixel_silu(const float* x, const float* gamma, const float* beta, void* y,
                                        int64_t batch, int64_t frames_per_seq, int64_t pixels, int64_t channels,
                                        float eps, int act_silu, int operand_mode, void* stream_v) {
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_groupnorm_pixel_silu", PN_OPERAND_BF16, PN_OPERAND_SPLIT3, PN_OPERAND_F32);
   PN_REQUIRE(x && gamma && beta && y, "pn_groupnorm_pixel_silu: null pointer");
   PN_REQUIRE(channels % 64 == 0, "pn_groupnorm_pixel_silu: C=%lld must be a multiple of 64", (long long)channels);
   PN_REQUIRE(batch > 0 && frames_per_seq > 0 && pixels > 0, "pn_groupnorm_pixel_silu: empty input");
-  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_groupnorm_pixel_silu: operand_mode %d", operand_mode);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   PN_REQUIRE(frames_per_seq <= 16, "pn_groupnorm_pixel_silu: T=%lld > 16 unsupported", (long long)frames_per_seq);
   const long long blocks = batch * pixels;
@@ -481,7 +482,7 @@ extern "C" int pn_groupnorm_pixel_silu(const float* x, const float* gamma, const
   const int threads = (int)frames_per_seq * 32;
   const int T = (int)frames_per_seq, P = (int)pixels, C = (int)channels;
   switch (C / 32) {
-#define PN_GNP_CASE(CPG) case CPG: PN_DISPATCH_OP(operand_mode, gn_pixel_kernel<CPG, OP><<<(unsigned)blocks, threads, 0, st>>>(x, gamma, beta, y, T, P, C, eps, act_silu)); break;
+#define PN_GNP_CASE(CPG) case CPG: PN_DISPATCH_OP(Modes, operand_mode, gn_pixel_kernel<CPG, OP><<<(unsigned)blocks, threads, 0, st>>>(x, gamma, beta, y, T, P, C, eps, act_silu)); break;
     PN_GNP_CASE(2) PN_GNP_CASE(4) PN_GNP_CASE(6) PN_GNP_CASE(8) PN_GNP_CASE(10) PN_GNP_CASE(12) PN_GNP_CASE(16) PN_GNP_CASE(20)
     PN_GNP_CASE(24) PN_GNP_CASE(30) PN_GNP_CASE(32) PN_GNP_CASE(40) PN_GNP_CASE(60) PN_GNP_CASE(80)
 #undef PN_GNP_CASE
@@ -495,13 +496,13 @@ extern "C" int pn_groupnorm_pixel_silu(const float* x, const float* gamma, const
 
 extern "C" int pn_layernorm(const void* x, int x_is_bf16, const float* gamma, const float* beta, void* y, int64_t rows,
                             int64_t channels, float eps, int operand_mode, void* stream_v) {
+  PN_OPERAND_MODES(Modes, operand_mode, "pn_layernorm", PN_OPERAND_BF16, PN_OPERAND_SPLIT3, PN_OPERAND_F32);
   PN_REQUIRE(x && gamma && beta && y, "pn_layernorm: null pointer");
   PN_REQUIRE(channels % 4 == 0 && channels <= 2048 && channels > 0, "pn_layernorm: C=%lld unsupported", (long long)channels);
   PN_REQUIRE(rows > 0, "pn_layernorm: empty input");
-  PN_REQUIRE(operand_mode >= 0 && operand_mode <= 2, "pn_layernorm: operand_mode %d", operand_mode);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   const int C = (int)channels;
-  if (x_is_bf16 && operand_mode == PN_OP_BF16 && C % 64 == 0) {
+  if (x_is_bf16 && operand_mode == PN_OPERAND_BF16 && C % 64 == 0) {
     // fast path: LPR lanes per row, NV = C / (8 LPR) loads per lane (5 for C = 320 / 640 / 1280)
 #define PN_LNB(LPR, NV)                                                                                                            \
     do {                                                                                                                           \
@@ -527,10 +528,10 @@ extern "C" int pn_layernorm(const void* x, int x_is_bf16, const float* gamma, co
 #define PN_LN(MAXV)                                                                                                          \
   do {                                                                                                                       \
     if (x_is_bf16)                                                                                                           \
-      PN_DISPATCH_OP(operand_mode, layernorm_kernel<MAXV, OP, __nv_bfloat16><<<(unsigned)blocks, 256, 0, st>>>(              \
+      PN_DISPATCH_OP(Modes, operand_mode, layernorm_kernel<MAXV, OP, __nv_bfloat16><<<(unsigned)blocks, 256, 0, st>>>(       \
           reinterpret_cast<const __nv_bfloat16*>(x), gamma, beta, y, rows, C, eps));                                         \
     else                                                                                                                     \
-      PN_DISPATCH_OP(operand_mode, layernorm_kernel<MAXV, OP, float><<<(unsigned)blocks, 256, 0, st>>>(                      \
+      PN_DISPATCH_OP(Modes, operand_mode, layernorm_kernel<MAXV, OP, float><<<(unsigned)blocks, 256, 0, st>>>(               \
           reinterpret_cast<const float*>(x), gamma, beta, y, rows, C, eps));                                                 \
   } while (0)
   if (C <= 512) PN_LN(4);

@@ -1,20 +1,13 @@
-// How a producer kernel writes the A operand of the GEMM that follows it.
-//
-//  PN_OP_BF16   : bf16 [rows, C]                     (the fast path: bf16 products, fp32 accumulation)
-//  PN_OP_SPLIT3 : bf16 [rows, 3C] = [hi | lo | hi]   (parity mode) with hi = bf16(v), lo = bf16(v - hi).
-//                 Against weights packed as [W_hi | W_hi | W_lo] per tap the SAME wgmma GEMM kernel computes
-//                 hi*W_hi + lo*W_hi + hi*W_lo = v*W up to the dropped lo*W_lo term (2^-18 relative): fp32-class
-//                 products on the bf16 tensor pipe by K-concatenation, no kernel change.
-//  PN_OP_F32    : fp32 [rows, C]                     (consumers that are CUDA-core kernels in parity mode)
-//  PN_OP_SPLIT3_B: bf16 [rows, 3C] = [hi | hi | lo]  (parity mode, the WEIGHT form of ops.split3 made on the device: the
-//                 B operand of a GEMM whose two factors are both activations, the VAE mid-block attention's S = q k^T
-//                 and O = P v). Only pn_cast_operand writes it; PN_DISPATCH_OP does not instantiate it.
+// How a producer kernel writes the A operand of the GEMM that follows it: in one of the layouts of pn_operand_mode
+// (include/panacea_b200.h), chosen by the kernel's OP template argument. In the split forms the GEMM drops the
+// lo*W_lo term of (hi + lo)(W_hi + W_lo): it is 2^-18 of the product, below fp32-class accuracy.
 #pragma once
+#include <type_traits>
+#include "common.cuh"
 #include "ptx.cuh"
+#include "../../include/panacea_b200.h"
 
 namespace pn {
-
-enum : int { PN_OP_BF16 = 0, PN_OP_SPLIT3 = 1, PN_OP_F32 = 2, PN_OP_SPLIT3_B = 3 };
 
 __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
   const __nv_bfloat16 ha = __float2bfloat16_rn(a), hb = __float2bfloat16_rn(b);
@@ -23,100 +16,87 @@ __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uin
   lo = pack_bf16x2(ra, rb);
 }
 
-// element size of the stored operand row in units of its own dtype
-template <int OP>
-__device__ __forceinline__ constexpr int op_row_mult() { return OP == PN_OP_SPLIT3 || OP == PN_OP_SPLIT3_B ? 3 : 1; }
-
-// 8 consecutive channels [col, col+8) of row `row` of a [rows, C] operand
-template <int OP>
-__device__ __forceinline__ void store_op8(void* base, size_t row, int C, int col, const float (&v)[8]) {
-  if (OP == PN_OP_F32) {
-    float* p = reinterpret_cast<float*>(base) + row * (size_t)C + col;
-    *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
-    *reinterpret_cast<float4*>(p + 4) = make_float4(v[4], v[5], v[6], v[7]);
-  } else if (OP == PN_OP_BF16) {
-    __nv_bfloat16* p = reinterpret_cast<__nv_bfloat16*>(base) + row * (size_t)C + col;
-    *reinterpret_cast<uint4*>(p) = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
-                                              pack_bf16x2(v[6], v[7]));
-  } else if (OP == PN_OP_SPLIT3_B) {
-    __nv_bfloat16* p = reinterpret_cast<__nv_bfloat16*>(base) + row * (size_t)(3 * C) + col;
-    uint32_t h[4], l[4];
+// N consecutive channels as one vector access: the bf16 vector of N values (`pack`, or `words` from N / 2 packed pairs),
+// and the fp32 vector (N <= 4; 8 channels are two float4 accesses). split() makes the hi and lo words of the split
+// forms; it is a loop for 8 channels and written out for 2 and 4 because the compiler schedules the callers differently
+// for the two forms, and these are the ones the producers' SASS was tuned with.
+template <int N> struct op_vec;
+template <> struct op_vec<2> {
+  using bf16 = uint32_t;
+  using f32 = float2;
+  static __device__ __forceinline__ bf16 words(const uint32_t* w) { return w[0]; }
+  static __device__ __forceinline__ bf16 pack(const float* v) { return pack_bf16x2(v[0], v[1]); }
+  static __device__ __forceinline__ f32 floats(const float* v) { return make_float2(v[0], v[1]); }
+  static __device__ __forceinline__ void split(const float* v, uint32_t* hi, uint32_t* lo) {
+    split_bf16x2(v[0], v[1], hi[0], lo[0]);
+  }
+};
+template <> struct op_vec<4> {
+  using bf16 = uint2;
+  using f32 = float4;
+  static __device__ __forceinline__ bf16 words(const uint32_t* w) { return make_uint2(w[0], w[1]); }
+  static __device__ __forceinline__ bf16 pack(const float* v) {
+    return make_uint2(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]));
+  }
+  static __device__ __forceinline__ f32 floats(const float* v) { return make_float4(v[0], v[1], v[2], v[3]); }
+  static __device__ __forceinline__ void split(const float* v, uint32_t* hi, uint32_t* lo) {
+    split_bf16x2(v[0], v[1], hi[0], lo[0]);
+    split_bf16x2(v[2], v[3], hi[1], lo[1]);
+  }
+};
+template <> struct op_vec<8> {
+  using bf16 = uint4;
+  static __device__ __forceinline__ bf16 words(const uint32_t* w) { return make_uint4(w[0], w[1], w[2], w[3]); }
+  static __device__ __forceinline__ bf16 pack(const float* v) {
+    return make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+  }
+  static __device__ __forceinline__ void split(const float* v, uint32_t* hi, uint32_t* lo) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) split_bf16x2(v[2 * i], v[2 * i + 1], h[i], l[i]);
-    const uint4 hv = make_uint4(h[0], h[1], h[2], h[3]);
-    *reinterpret_cast<uint4*>(p) = hv;
-    *reinterpret_cast<uint4*>(p + C) = hv;
-    *reinterpret_cast<uint4*>(p + 2 * C) = make_uint4(l[0], l[1], l[2], l[3]);
+    for (int i = 0; i < 4; ++i) split_bf16x2(v[2 * i], v[2 * i + 1], hi[i], lo[i]);
+  }
+};
+
+// N = 2, 4 or 8 consecutive channels [col, col + N) of row `row` of a [rows, C] operand
+template <int OP, int N>
+__device__ __forceinline__ void store_op(void* base, size_t row, int C, int col, const float (&v)[N]) {
+  using V = op_vec<N>;
+  using B = typename V::bf16;
+  if constexpr (OP == PN_OPERAND_BF16) {
+    *reinterpret_cast<B*>(reinterpret_cast<__nv_bfloat16*>(base) + row * (size_t)C + col) = V::pack(v);
+  } else if constexpr (OP == PN_OPERAND_F32) {
+    using F = op_vec<N < 4 ? N : 4>;
+    using T = typename F::f32;
+    *reinterpret_cast<T*>(reinterpret_cast<float*>(base) + row * (size_t)C + col) = F::floats(v);
+    if constexpr (N == 8) *reinterpret_cast<T*>(reinterpret_cast<float*>(base) + row * (size_t)C + col + 4) = F::floats(v + 4);
   } else {
     __nv_bfloat16* p = reinterpret_cast<__nv_bfloat16*>(base) + row * (size_t)(3 * C) + col;
-    uint32_t h[4], l[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) split_bf16x2(v[2 * i], v[2 * i + 1], h[i], l[i]);
-    const uint4 hv = make_uint4(h[0], h[1], h[2], h[3]);
-    *reinterpret_cast<uint4*>(p) = hv;
-    *reinterpret_cast<uint4*>(p + C) = make_uint4(l[0], l[1], l[2], l[3]);
-    *reinterpret_cast<uint4*>(p + 2 * C) = hv;
+    uint32_t hi[N / 2], lo[N / 2];
+    V::split(v, hi, lo);
+    constexpr bool a_form = OP == PN_OPERAND_SPLIT3;
+    *reinterpret_cast<B*>(p) = V::words(hi);
+    *reinterpret_cast<B*>(p + C) = V::words(a_form ? lo : hi);
+    *reinterpret_cast<B*>(p + 2 * C) = V::words(a_form ? hi : lo);
   }
 }
 
-template <int OP>
-__device__ __forceinline__ void store_op4(void* base, size_t row, int C, int col, const float (&v)[4]) {
-  if (OP == PN_OP_F32) {
-    *reinterpret_cast<float4*>(reinterpret_cast<float*>(base) + row * (size_t)C + col) = make_float4(v[0], v[1], v[2], v[3]);
-  } else if (OP == PN_OP_BF16) {
-    *reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(base) + row * (size_t)C + col) =
-        make_uint2(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]));
-  } else if (OP == PN_OP_SPLIT3_B) {
-    __nv_bfloat16* p = reinterpret_cast<__nv_bfloat16*>(base) + row * (size_t)(3 * C) + col;
-    uint32_t h0, h1, l0, l1;
-    split_bf16x2(v[0], v[1], h0, l0);
-    split_bf16x2(v[2], v[3], h1, l1);
-    *reinterpret_cast<uint2*>(p) = make_uint2(h0, h1);
-    *reinterpret_cast<uint2*>(p + C) = make_uint2(h0, h1);
-    *reinterpret_cast<uint2*>(p + 2 * C) = make_uint2(l0, l1);
-  } else {
-    __nv_bfloat16* p = reinterpret_cast<__nv_bfloat16*>(base) + row * (size_t)(3 * C) + col;
-    uint32_t h0, h1, l0, l1;
-    split_bf16x2(v[0], v[1], h0, l0);
-    split_bf16x2(v[2], v[3], h1, l1);
-    *reinterpret_cast<uint2*>(p) = make_uint2(h0, h1);
-    *reinterpret_cast<uint2*>(p + C) = make_uint2(l0, l1);
-    *reinterpret_cast<uint2*>(p + 2 * C) = make_uint2(h0, h1);
+// The operand modes an entry point accepts. PN_OPERAND_MODES(Name, mode, "entry", modes...) declares them as the type
+// Name and returns PN_ERR_INVALID for any other mode; an entry point states it before it does any work.
+// PN_DISPATCH_OP(Name, mode, launch) then instantiates the launch expression, which names the mode OP, for exactly
+// these modes and runs the one that matches.
+template <int... MODES>
+struct OperandModes {
+  static constexpr bool has(int mode) { return ((mode == MODES) || ...); }
+  template <typename F>
+  static void dispatch(int mode, F&& launch) {
+    ((mode == MODES ? launch(std::integral_constant<int, MODES>{}) : void()), ...);
   }
-}
+};
 
-template <int OP>
-__device__ __forceinline__ void store_op2(void* base, size_t row, int C, int col, float a, float b) {
-  if (OP == PN_OP_F32) {
-    *reinterpret_cast<float2*>(reinterpret_cast<float*>(base) + row * (size_t)C + col) = make_float2(a, b);
-  } else if (OP == PN_OP_BF16) {
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(base) + row * (size_t)C + col) = pack_bf16x2(a, b);
-  } else if (OP == PN_OP_SPLIT3_B) {
-    __nv_bfloat16* p = reinterpret_cast<__nv_bfloat16*>(base) + row * (size_t)(3 * C) + col;
-    uint32_t h, l;
-    split_bf16x2(a, b, h, l);
-    *reinterpret_cast<uint32_t*>(p) = h;
-    *reinterpret_cast<uint32_t*>(p + C) = h;
-    *reinterpret_cast<uint32_t*>(p + 2 * C) = l;
-  } else {
-    __nv_bfloat16* p = reinterpret_cast<__nv_bfloat16*>(base) + row * (size_t)(3 * C) + col;
-    uint32_t h, l;
-    split_bf16x2(a, b, h, l);
-    *reinterpret_cast<uint32_t*>(p) = h;
-    *reinterpret_cast<uint32_t*>(p + C) = l;
-    *reinterpret_cast<uint32_t*>(p + 2 * C) = h;
-  }
-}
+#define PN_OPERAND_MODES(Name, mode, entry, ...)    \
+  using Name = ::pn::OperandModes<__VA_ARGS__>;     \
+  PN_REQUIRE(Name::has(mode), entry ": operand_mode %d unsupported", (int)(mode))
 
-// dispatch a kernel launch expression on a run-time operand mode (BF16 / SPLIT3 / F32). Any other mode, SPLIT3_B
-// included, makes the enclosing entry point return an error: a producer that forgets its own operand_mode check still
-// never writes an operand of the wrong size.
-#define PN_DISPATCH_OP(mode, ...)                                                           \
-  do {                                                                                      \
-    if ((mode) == ::pn::PN_OP_BF16) { constexpr int OP = ::pn::PN_OP_BF16; __VA_ARGS__; }   \
-    else if ((mode) == ::pn::PN_OP_SPLIT3) { constexpr int OP = ::pn::PN_OP_SPLIT3; __VA_ARGS__; } \
-    else if ((mode) == ::pn::PN_OP_F32) { constexpr int OP = ::pn::PN_OP_F32; __VA_ARGS__; } \
-    else return ::pn::fail(::pn::PN_ERR_INVALID, "operand_mode %d is not a producer store mode", (int)(mode)); \
-  } while (0)
+#define PN_DISPATCH_OP(MODES, mode, ...) \
+  MODES::dispatch((mode), [&](auto op_) { constexpr int OP = decltype(op_)::value; __VA_ARGS__; })
 
 }  // namespace pn

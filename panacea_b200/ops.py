@@ -43,15 +43,21 @@ def geglu_pack(t: torch.Tensor) -> torch.Tensor:
     return torch.stack([v, g], 1).reshape(t.shape).contiguous()
 
 
+def split_encode(x: torch.Tensor, weight_form: bool = False) -> torch.Tensor:
+    """fp32 [..., C] -> bf16 [..., 3C] with hi = bf16(x), lo = bf16(x - hi): the A form [hi | lo | hi] producers store
+    (OP_SPLIT3), or with `weight_form` [hi | hi | lo] (OP_SPLIT3_B, the form split3 packs weights in)."""
+    x = x.detach().to(F32)
+    hi = x.to(BF16)
+    lo = (x - hi.to(F32)).to(BF16)
+    return torch.cat([hi, hi, lo] if weight_form else [hi, lo, hi], dim=-1)
+
+
 def split3(t: torch.Tensor, taps: int = 1) -> torch.Tensor:
     """Parity-mode packing of a WEIGHT matrix [N, taps*C] (fp32) -> bf16 [N, taps*3C]: per tap [W_hi | W_hi | W_lo] with
-    W_hi = bf16(W), W_lo = bf16(W - W_hi). Against an activation operand stored [a_hi | a_lo | a_hi] (operand.cuh)
+    W_hi = bf16(W), W_lo = bf16(W - W_hi). Against an activation operand stored [a_hi | a_lo | a_hi] (split_encode)
     the bf16 GEMM then computes a_hi W_hi + a_lo W_hi + a_hi W_lo = a W up to 2^-18 relative."""
     n, k = t.shape
-    w = t.detach().to(F32).reshape(n, taps, k // taps)
-    hi = w.to(BF16)
-    lo = (w - hi.to(F32)).to(BF16)
-    return torch.cat([hi, hi, lo], dim=2).reshape(n, 3 * k).contiguous()
+    return split_encode(t.reshape(n, taps, k // taps), weight_form=True).reshape(n, 3 * k).contiguous()
 
 
 def _attn_args(q, k, v, out, *, q_ld, kv_ld, F, H, V, W, Hk, Vk, Wk, heads, head_dim, views):

@@ -27,6 +27,7 @@ from pathlib import Path
 import numpy as np
 import torch
 
+from panacea_b200.ops import split_encode
 from torch_ref_ops import TorchRefOps64
 
 F32, BF16, F64 = torch.float32, torch.bfloat16, torch.float64
@@ -86,11 +87,9 @@ def _encode(x, fmt):
     x = x.float()
     if fmt == "f32":
         return x
-    hi = x.to(BF16)
     if fmt == "bf16":
-        return hi
-    lo = (x - hi.float()).to(BF16)
-    return torch.cat([hi, lo, hi] if fmt == "split3" else [hi, hi, lo], dim=-1)
+        return x.to(BF16)
+    return split_encode(x, weight_form=fmt == "split3b")
 
 
 def _bits(t):

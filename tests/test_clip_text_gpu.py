@@ -8,6 +8,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from op_check import _decode
 from tools.make_clip_golden import clip_text_weights, golden_subset
 
 pytestmark = pytest.mark.gpu
@@ -47,7 +48,7 @@ def test_attention_causal_f32_kernel(L, b):
     g = torch.Generator().manual_seed(L * 10 + b + 1)
     qkv = torch.randn(b, L, 3 * 1024, generator=g) * 2
     out = ParityOps().attention_causal(qkv.cuda(), 16).cpu()             # split3 operand [hi | lo | hi]
-    dec = out[..., :1024].float() + out[..., 1024:2048].float()
+    dec = _decode(out, "split3")
     ref = _causal_ref(qkv.double(), 16).float()
     rel = ((dec - ref).norm() / ref.norm()).item()
     assert rel <= 1e-5, rel

@@ -12,7 +12,7 @@ from oracle.make_golden import VAE_DDCONFIG, vae_decoder_input, vae_decoder_weig
 from panacea_b200.vae import VAEDecoderEngine, VAEEncoderEngine, decoder_param_spec, encoder_param_spec
 from test_eps_parity_gpu import BOUNDS
 from tools.make_vae_golden import FULL_WIDTH_DDCONFIG, full_width_inputs
-from torch_ref_ops import TorchSplitOps, _enc_weight_form
+from torch_ref_ops import TorchSplitOps
 
 GOLDEN = Path(__file__).resolve().parent / "golden"
 
@@ -66,7 +66,7 @@ def test_full_width_golden_keys_are_the_engine_specs():
 def test_weight_form_emulation_is_split3():
     from panacea_b200.ops import split3
     w = torch.randn(24, 40, generator=torch.Generator().manual_seed(5))
-    assert torch.equal(_enc_weight_form(w), split3(w))
+    assert torch.equal(TorchSplitOps().cast_operand(w, weight_form=True), split3(w))
 
 
 def _wrapper(**kw):

@@ -9,6 +9,7 @@ from pathlib import Path
 import pytest
 import torch
 
+from op_check import _decode
 from oracle.make_golden import VAE_DDCONFIG, vae_decoder_input, vae_decoder_weights, vae_encoder_input
 from panacea_b200.vae import decoder_param_spec, encoder_param_spec
 from test_eps_parity_gpu import _report
@@ -33,14 +34,13 @@ def _wrapper(dd, precision=None, sd=None, **kw):
 
 # ------------------------------------------------------------------------------------------------ kernels
 def test_weight_form_cast_is_host_split3():
-    from panacea_b200.ops import ParityOps, split3
-    from torch_ref_ops import _enc
+    from panacea_b200.ops import ParityOps, split3, split_encode
     ops = ParityOps()
     for rows, cols in ((300, 520), (64, 12288), (7, 4)):
         w = torch.randn(rows, cols, generator=torch.Generator().manual_seed(rows)) * 3.0
         got = ops.cast_operand(w.cuda(), weight_form=True).cpu()
         assert torch.equal(got, split3(w)), (rows, cols)
-        assert torch.equal(ops.cast_operand(w.cuda()).cpu(), _enc(w)), (rows, cols)
+        assert torch.equal(ops.cast_operand(w.cuda()).cpu(), split_encode(w)), (rows, cols)
 
 
 def _softmax_operand(lib, s, mode, out, scale):
@@ -61,10 +61,8 @@ def test_softmax_rows_operand(rows, N):
     assert torch.equal(got_bf16, ref_bf16), "bf16 mode must be bitwise NativeOps.softmax_rows"
     p3 = pops.softmax_rows(s, scale)
     assert p3.shape == (rows, 3 * N) and p3.dtype == torch.bfloat16
-    hi, lo, hi2 = p3.float().split(N, dim=-1)
-    assert torch.equal(hi, hi2)
     ref = torch.softmax(s.double() * scale, dim=-1)
-    rel = ((hi.double() + lo.double() - ref).abs() / ref).max().item()
+    rel = ((_decode(p3, "split3") - ref).abs() / ref).max().item()
     assert rel <= 1e-5, rel
 
 

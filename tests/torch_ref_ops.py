@@ -12,6 +12,8 @@ import math
 import torch
 import torch.nn.functional as F
 
+from panacea_b200.ops import split3, split_encode
+
 F32 = torch.float32
 
 
@@ -259,20 +261,6 @@ class TorchFoldOps(TorchRefOps):
     LN_FOLD_MAX_C = 640
 
 
-def _enc(x):
-    """operand.cuh PN_OP_SPLIT3: fp32 [..., C] -> bf16 [..., 3C] = [hi | lo | hi]."""
-    hi = x.to(torch.bfloat16)
-    lo = (x - hi.float()).to(torch.bfloat16)
-    return torch.cat([hi, lo, hi], dim=-1)
-
-
-def _enc_weight_form(x):
-    """operand.cuh PN_OP_SPLIT3_B: fp32 [..., C] -> bf16 [..., 3C] = [hi | hi | lo], the layout split3() packs weights in."""
-    hi = x.to(torch.bfloat16)
-    lo = (x - hi.float()).to(torch.bfloat16)
-    return torch.cat([hi, hi, lo], dim=-1)
-
-
 class TorchSplitOps(TorchRefOps):
     """CPU emulation of panacea_b200.ops.ParityOps: producers store split-bf16 operands [hi | lo | hi], weights are
     packed [W_hi | W_hi | W_lo] by the product's own split3(), and the GEMM multiplies the bf16 VALUES exactly as the
@@ -282,51 +270,50 @@ class TorchSplitOps(TorchRefOps):
     operand_mult = 3
 
     def pack_matrix(self, w, taps=1):
-        from panacea_b200.ops import split3
         return split3(w, taps)
 
     def gemm(self, a, w, *, geglu=False, out_dtype=F32, **kw):
         y = super().gemm(a, w, geglu=geglu, out_dtype=F32, **kw)
-        return _enc(y) if geglu else y
+        return split_encode(y) if geglu else y
 
     def groupnorm(self, x, gamma, beta, eps, silu, want_raw=False, out_f32=False):
         r = super().groupnorm(x, gamma, beta, eps, silu, want_raw)
         if out_f32:
             return r
-        return (_enc(r[0]), _enc(r[1])) if want_raw else _enc(r)
+        return (split_encode(r[0]), split_encode(r[1])) if want_raw else split_encode(r)
 
     def groupnorm_pixel(self, *a, **k):
-        return _enc(super().groupnorm_pixel(*a, **k))
+        return split_encode(super().groupnorm_pixel(*a, **k))
 
     def layernorm(self, x, gamma, beta, eps=1e-5, out_f32=False):
         y = super().layernorm(x, gamma, beta, eps)
-        return y if out_f32 else _enc(y)
+        return y if out_f32 else split_encode(y)
 
     def attention_view(self, *a, **k):
-        return _enc(super().attention_view(*a, **k))
+        return split_encode(super().attention_view(*a, **k))
 
     def attention_text(self, *a, **k):
-        return _enc(super().attention_text(*a, **k))
+        return split_encode(super().attention_text(*a, **k))
 
     def attention_temporal(self, *a, **k):
-        return _enc(super().attention_temporal(*a, **k))
+        return split_encode(super().attention_temporal(*a, **k))
 
     def attention_causal(self, *a, **k):
-        return _enc(super().attention_causal(*a, **k))
+        return split_encode(super().attention_causal(*a, **k))
 
     def gelu_operand(self, x):
-        return _enc(super().gelu_operand(x))
+        return split_encode(super().gelu_operand(x))
 
     def im2col_s2(self, x, pad=1):
         cols, geo = super().im2col_s2(x, pad)
         C = x.shape[-1]
-        return _enc(cols.reshape(cols.shape[0], 9, C)).reshape(cols.shape[0], 27 * C), geo
+        return split_encode(cols.reshape(cols.shape[0], 9, C)).reshape(cols.shape[0], 27 * C), geo
 
     def upsample2x(self, x):
-        return _enc(super().upsample2x(x))
+        return split_encode(super().upsample2x(x))
 
     def cast_operand(self, x, weight_form=False):
-        return _enc_weight_form(x) if weight_form else _enc(x)
+        return split_encode(x, weight_form)
 
     def softmax_rows(self, s, scale):
-        return _enc(super().softmax_rows(s, scale))
+        return split_encode(super().softmax_rows(s, scale))

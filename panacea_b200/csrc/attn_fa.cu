@@ -11,12 +11,21 @@
 // (Temporal self-attention over T<=16 frames is a CUDA-core kernel, attn_small.cu.)
 //
 // CTA = one query tile (<= 128 queries of one frame/view/head), 288 threads:
-//   warps 0-3 / 4-7: two consumer warpgroups, query rows 0-63 / 64-127. Per key block of <= 128 keys:
-//                    S = Q K^T   wgmma m64n128k16, Q and K K-major from shared memory (fp32 S in registers);
+//   warps 0-3 / 4-7: two consumer warpgroups, query rows 0-63 / 64-127. Per key block of <= N keys:
+//                    S = Q K^T   wgmma m64nNk16, Q and K K-major from shared memory (fp32 S in registers);
 //                    online softmax in registers (a query row lives in the 4 lanes of a quad);
-//                    O += P V    wgmma m64n64k16 with P as the REGISTER A operand (the S accumulator fragment is the
-//                                A fragment layout) and V the MN-major B operand from shared memory.
+//                    O += P V    N / 16 wgmma m64n64k16 with P as the REGISTER A operand (the S accumulator fragment is
+//                                the A fragment layout) and V the MN-major B operand from shared memory.
+//                    S of block j + 1 and P V of block j issue as one run of wgmmas and retire together (one wait
+//                    per block, not two); the softmax of block j + 1 runs while the other warpgroup's MMAs use the
+//                    tensor cores. (A wait<1> between the two, meant to run the exponentials under P V of the same
+//                    warpgroup, is moved by ptxas ahead of them, so the kernel does not pretend to have one.)
 //   warp 8:          TMA producer (Q once, K and V boxes through a STAGES-deep mbarrier ring).
+// N, the width of the S wgmma, is the key block's row count rounded up to 16 (every block of a call has the same count:
+// kh divides Hk), so no MMA, exponential or mask runs on keys that do not exist beyond that rounding. Query tiles are a
+// rectangle of the view (qw x qh tokens) or, where a rectangle of whole rows would leave MMA rows empty and the view width
+// is a multiple of 8, 128 consecutive tokens of the view in row-major order, loaded as 8-token boxes (one 1024 B
+// swizzle atom each, so the tile lands in shared memory exactly as one 128-row box would).
 // head_dim 80 is a 64-channel part plus a 16-channel part (a TMA box with a 128 B swizzle cannot be wider than 64
 // bf16): every Q/K/V tile has a second, 32 B-row tile; S gets a fifth K = 16 step on the 16-channel tiles and
 // O = P V a second wgmma of N = 16 per key step into output channels 64..79.
@@ -30,7 +39,8 @@ namespace pn {
 constexpr int FA_THREADS = 288;
 constexpr int FA_TILE_BYTES = 128 * 128;          // 128 rows x 64 bf16 (128 B rows, 128B swizzle)
 constexpr int FA_XTILE_BYTES = 128 * 32;          // head_dim 80: the channels 64..79 of 128 rows (32 B rows, 32B swizzle)
-constexpr int FA_MAX_KEYS = 128;                  // keys per block = the N of the S wgmma
+constexpr int FA_MAX_KEYS = 128;                  // keys per block: the largest N of the S wgmma
+constexpr int FA_QBOX = 8;                        // tokens per Q box of a row-major query tile
 
 template <int D>
 struct FaL {
@@ -51,6 +61,7 @@ struct FaParams {
   CUtensorMap mapQx, mapKx, mapVx;   // head_dim 80: 16-channel boxes (32B swizzle) of the same tensors
   int heads;
   int F, H, V, W;              // query token grid
+  int q_rowmajor;              // 1: query tile ti = tokens [128 ti, 128 ti + 128) of the view, row-major; 0: a qw x qh rectangle
   int qw, qh, tiles_x, tiles_y;
   int tiles_per_group;         // query tiles of one (frame, view, head)
   int kw, kh, kv_rows, kv_yblocks;
@@ -62,10 +73,13 @@ struct FaParams {
   long long out_ld;            // token stride of out (elements)
 };
 
-template <int D>
+template <int D, int N>
 __global__ void __launch_bounds__(FA_THREADS, 1) attn_fa_kernel(const __grid_constant__ FaParams p) {
+  static_assert(N % 16 == 0 && N >= 16 && N <= FA_MAX_KEYS, "a key block is a whole number of K = 16 steps of P V");
   using L = FaL<D>;
   constexpr int STAGES = L::STAGES;
+  constexpr int GROUPS = N / 8;                  // 8-key column groups of the S fragment
+  constexpr int KSTEPS = N / 16;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::BAR);
@@ -76,7 +90,7 @@ __global__ void __launch_bounds__(FA_THREADS, 1) attn_fa_kernel(const __grid_con
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  // zero Q/K/V staging once: rows a TMA box does not cover (keys kv_rows..127, queries beyond the tile) must read as 0,
+  // zero Q/K/V staging once: rows a TMA box does not cover (keys kv_rows..N-1, queries beyond the tile) must read as 0,
   // never as stale NaNs
   {
     uint4* z = reinterpret_cast<uint4*>(smem);
@@ -100,16 +114,28 @@ __global__ void __launch_bounds__(FA_THREADS, 1) attn_fa_kernel(const __grid_con
 
   if (warp == 8) {
     // ===================== TMA producer (warp-wide loop, TMA issue under elect.sync) =====================
-    const uint32_t q_bytes = (uint32_t)(p.qw * p.qh) * (D == 80 ? 160u : 128u);
-    const uint32_t kv_bytes = (uint32_t)p.kv_rows * (D == 80 ? 160u : 128u);
+    const uint32_t row_bytes = D == 80 ? 160u : 128u;
+    const uint32_t kv_bytes = (uint32_t)p.kv_rows * row_bytes;
     if (elect_one()) {
       tma_prefetch_desc(&p.mapQ);
       tma_prefetch_desc(&p.mapK);
       tma_prefetch_desc(&p.mapV);
-      mbar_arrive_expect_tx(q_full, q_bytes);
-      const int x0 = (ti % p.tiles_x) * p.qw, y0 = (ti / p.tiles_x) * p.qh;
-      tma_load_5d(smem + L::Q, &p.mapQ, q_full, head * D, x0, view, y0, frame);
-      if (D == 80) tma_load_5d(smem + L::QX, &p.mapQx, q_full, head * D + 64, x0, view, y0, frame);
+      if (p.q_rowmajor) {
+        // W % 8 == 0, so an 8-token box never crosses a view row and the tile's last box is either full or absent
+        const int t0 = ti * 128;
+        const int rows = min(128, p.H * p.W - t0);
+        mbar_arrive_expect_tx(q_full, (uint32_t)rows * row_bytes);
+        for (int r = 0; r < rows; r += FA_QBOX) {
+          const int y = (t0 + r) / p.W, x = t0 + r - y * p.W;
+          tma_load_5d(smem + L::Q + r * 128, &p.mapQ, q_full, head * D, x, view, y, frame);
+          if (D == 80) tma_load_5d(smem + L::QX + r * 32, &p.mapQx, q_full, head * D + 64, x, view, y, frame);
+        }
+      } else {
+        mbar_arrive_expect_tx(q_full, (uint32_t)(p.qw * p.qh) * row_bytes);
+        const int x0 = (ti % p.tiles_x) * p.qw, y0 = (ti / p.tiles_x) * p.qh;
+        tma_load_5d(smem + L::Q, &p.mapQ, q_full, head * D, x0, view, y0, frame);
+        if (D == 80) tma_load_5d(smem + L::QX, &p.mapQx, q_full, head * D + 64, x0, view, y0, frame);
+      }
     }
     const int kv_frame = frame / p.kv_frame_div;
     int vi = 0, yb = 0;
@@ -144,85 +170,114 @@ __global__ void __launch_bounds__(FA_THREADS, 1) attn_fa_kernel(const __grid_con
   const uint64_t dVx0 = wgmma_desc(base + L::KV + 2 * FA_TILE_BYTES + L::XB, 256, 256, kSw32);
   constexpr uint64_t STAGE_STEP = L::STAGE_BYTES >> 4;          // start-address field is in 16-byte units
   const float c = p.scale_log2;
-  const bool mask = p.kv_rows < FA_MAX_KEYS;
+  // keys kv_rows..N-1 exist only when kv_rows % 16 != 0, and then only in the last two 8-key groups
+  const bool mask = p.kv_rows < N;
 
   float o[32], ox[8];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < 8; ++i) ox[i] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // rows r and r + 8 of this thread
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // raw-logit maximum and row sum, rows r and r + 8
+  float s[N / 2];                                                   // S, then P, of the current block
+  uint32_t pa[KSTEPS][4];                                           // P as the A fragments of the K = 16 key steps
+  float alpha[2];                                                   // rescale of O and l for the block in s
 
-  mbar_wait(q_full, 0);
-  for (int j = 0; j < nblk; ++j) {
-    const int st = j % STAGES;
-    mbar_wait(&kv_full[st], (uint32_t)((j / STAGES) & 1));
-    float s[64];
-    wgmma_fence();
+  auto issue_s = [&](int st) {
 #pragma unroll
-    for (int k = 0; k < 4; ++k) wgmma_ss<128>(s, dQ + 2 * k, dK0 + STAGE_STEP * st + 2 * k, k > 0 ? 1u : 0u);
-    if (D == 80) wgmma_ss<128>(s, dQx, dKx0 + STAGE_STEP * st, 1u);
+    for (int k = 0; k < 4; ++k) wgmma_ss<N>(s, dQ + 2 * k, dK0 + STAGE_STEP * st + 2 * k, k > 0 ? 1u : 0u);
+    if (D == 80) wgmma_ss<N>(s, dQx, dKx0 + STAGE_STEP * st, 1u);
     wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(s);
-
-    // scaled logits (log2 domain), padding keys -> -inf; row maximum over the quad
+  };
+  auto issue_pv = [&](int st) {
+#pragma unroll
+    for (int kk = 0; kk < KSTEPS; ++kk) {      // 16 keys per step: 16 rows (128 B each) of V
+      wgmma_rs_tb<64>(o, pa[kk], dV0 + STAGE_STEP * st + kk * (2048 >> 4), 1u);
+      if (D == 80) wgmma_rs_tb<16>(ox, pa[kk], dVx0 + STAGE_STEP * st + kk * (512 >> 4), 1u);
+    }
+    wgmma_commit();
+  };
+  // online softmax of the raw logits in s: running maximum and sum, alpha, and s <- exp2(c * (s - m))
+  auto softmax = [&]() {
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-    for (int jj = 0; jj < 16; ++jj) {
+    for (int jj = 0; jj < GROUPS; ++jj) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        float v = s[4 * jj + e] * c;
-        if (mask && 8 * jj + 2 * quad + (e & 1) >= p.kv_rows) v = -INFINITY;
-        s[4 * jj + e] = v;
-        mx[e >> 1] = fmaxf(mx[e >> 1], v);
+        if (jj >= GROUPS - 2 && mask && 8 * jj + 2 * quad + (e & 1) >= p.kv_rows) s[4 * jj + e] = -INFINITY;
+        mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * jj + e]);
       }
     }
-    float alpha[2];
+    float mc[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
       mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
       const float m_new = fmaxf(m_run[h], mx[h]);
-      alpha[h] = ex2_approx(m_run[h] - m_new);                  // first block: exp2(-inf) = 0
+      alpha[h] = ex2_approx((m_run[h] - m_new) * c);              // first block: exp2(-inf) = 0
       m_run[h] = m_new;
+      mc[h] = m_new * c;
     }
     float rs[2] = {0.f, 0.f};
-    uint32_t pa[8][4];                                           // P as the A fragments of 8 K = 16 key steps
 #pragma unroll
-    for (int jj = 0; jj < 16; ++jj) {
+    for (int jj = 0; jj < GROUPS; ++jj) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float e0 = ex2_approx(s[4 * jj + 2 * h] - m_run[h]);
-        const float e1 = ex2_approx(s[4 * jj + 2 * h + 1] - m_run[h]);
-        rs[h] += e0 + e1;
-        pa[jj >> 1][(jj & 1) * 2 + h] = pack_bf16x2(e0, e1);
+      for (int e = 0; e < 4; ++e) {
+        const float x = fmaf(s[4 * jj + e], c, -mc[e >> 1]);      // scale and max-subtract in one FFMA
+        const float v = ex2_approx(x);
+        s[4 * jj + e] = v;
+        rs[e >> 1] += v;
       }
     }
 #pragma unroll
     for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + rs[h];
+  };
+  // O *= alpha, then P -> bf16 A fragments
+  auto rescale_and_pack = [&]() {
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) o[4 * jj + e] *= alpha[e >> 1];
-    }
+    for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
     if (D == 80) {
 #pragma unroll
-      for (int e = 0; e < 8; ++e) ox[e] *= alpha[(e >> 1) & 1];
+      for (int i = 0; i < 8; ++i) ox[i] *= alpha[(i >> 1) & 1];
     }
-
-    wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {      // 16 keys per step: 16 rows (128 B each) of V
-      wgmma_rs_tb<64>(o, pa[kk], dV0 + STAGE_STEP * st + kk * (2048 >> 4), 1u);
-      if (D == 80) wgmma_rs_tb<16>(ox, pa[kk], dVx0 + STAGE_STEP * st + kk * (512 >> 4), 1u);
+    for (int jj = 0; jj < GROUPS; ++jj) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) pa[jj >> 1][(jj & 1) * 2 + h] = pack_bf16x2(s[4 * jj + 2 * h], s[4 * jj + 2 * h + 1]);
     }
-    wgmma_commit();
-    wgmma_wait<0>();
+  };
+  auto pv_retired = [&](int st) {
     wgmma_fence_regs(o);
     if (D == 80) wgmma_fence_regs(ox);
-    if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[st]);   // both of this warpgroup's wgmma groups have retired
+#pragma unroll
+    for (int kk = 0; kk < KSTEPS; ++kk) wgmma_fence_regs(pa[kk]);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[st]);   // this warpgroup's reads of the stage have retired
+  };
+
+  mbar_wait(q_full, 0);
+  mbar_wait(&kv_full[0], 0);
+  wgmma_fence();
+  issue_s(0);
+  wgmma_wait<0>();
+  wgmma_fence_regs(s);
+  softmax();
+  rescale_and_pack();
+  for (int j = 1; j < nblk; ++j) {
+    const int st = j % STAGES, prev = (j - 1) % STAGES;
+    mbar_wait(&kv_full[st], (uint32_t)((j / STAGES) & 1));
+    wgmma_fence();
+    issue_s(st);
+    issue_pv(prev);
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    pv_retired(prev);
+    softmax();
+    rescale_and_pack();
   }
+  wgmma_fence();
+  issue_pv((nblk - 1) % STAGES);
+  wgmma_wait<0>();
+  pv_retired((nblk - 1) % STAGES);
 
   // normalise by the row sums and store this thread's two query rows (bf16)
 #pragma unroll
@@ -232,9 +287,18 @@ __global__ void __launch_bounds__(FA_THREADS, 1) attn_fa_kernel(const __grid_con
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv = 1.f / l;
     const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
-    const int yy = row / p.qw, xx = row - yy * p.qw;
-    const int x = (ti % p.tiles_x) * p.qw + xx, y = (ti / p.tiles_x) * p.qh + yy;
-    if (row >= p.qw * p.qh || x >= p.W || y >= p.H) continue;
+    int x, y;
+    if (p.q_rowmajor) {
+      const int t = ti * 128 + row;
+      y = t / p.W;
+      x = t - y * p.W;
+    } else {
+      if (row >= p.qw * p.qh) continue;
+      const int yy = row / p.qw, xx = row - yy * p.qw;
+      x = (ti % p.tiles_x) * p.qw + xx;
+      y = (ti / p.tiles_x) * p.qh + yy;
+    }
+    if (x >= p.W || y >= p.H) continue;
     const long long token = (((long long)frame * p.H + y) * p.V + view) * p.W + x;
     __nv_bfloat16* dst = p.out + token * p.out_ld + head * D + 2 * quad;
 #pragma unroll
@@ -247,6 +311,12 @@ __global__ void __launch_bounds__(FA_THREADS, 1) attn_fa_kernel(const __grid_con
     }
   }
 }
+
+// indexed by N / 16 - 1
+template <int D>
+void (*const fa_kernels[FA_MAX_KEYS / 16])(FaParams) = {attn_fa_kernel<D, 16>, attn_fa_kernel<D, 32>, attn_fa_kernel<D, 48>,
+                                                        attn_fa_kernel<D, 64>, attn_fa_kernel<D, 80>, attn_fa_kernel<D, 96>,
+                                                        attn_fa_kernel<D, 112>, attn_fa_kernel<D, 128>};
 
 }  // namespace pn
 
@@ -269,13 +339,15 @@ extern "C" int pn_attention(const pn_attn_args* a, int operand_mode, void* strea
   std::memset(&p, 0, sizeof(p));
   p.heads = a->heads;
   p.F = (int)a->F; p.H = (int)a->H; p.V = (int)a->V; p.W = (int)a->W;
-  // query tile: full view width when it fits, as many rows as keep <= 128 queries
+  // query tile: full view width when it fits, as many rows as keep <= 128 queries; 128 row-major tokens instead where
+  // such a rectangle would leave rows of the 128-row MMA tile empty and 8-token boxes tile the view rows
   p.qw = (int)(a->W <= 128 ? a->W : 128);
   p.qh = 128 / p.qw;
   if (p.qh > a->H) p.qh = (int)a->H;
   if (p.qh < 1) p.qh = 1;
   p.tiles_x = (int)((a->W + p.qw - 1) / p.qw);
   p.tiles_y = (int)((a->H + p.qh - 1) / p.qh);
+  p.q_rowmajor = a->W % FA_QBOX == 0 && a->W < 128 && p.qw * p.qh < 128 && a->H > p.qh;
   // key block: full key-view width (must fit one block row-wise), rows = largest divisor of Hk with <= 128 keys
   PN_REQUIRE(a->Wk <= FA_MAX_KEYS, "pn_attention: key view width %lld > %d unsupported", (long long)a->Wk, FA_MAX_KEYS);
   p.kw = (int)a->Wk;
@@ -304,11 +376,12 @@ extern "C" int pn_attention(const pn_attn_args* a, int operand_mode, void* strea
     const uint64_t dims[5] = {chq, (uint64_t)a->W, (uint64_t)a->V, (uint64_t)a->H, (uint64_t)a->F};
     const uint64_t ld = (uint64_t)a->q_ld;
     const uint64_t str[4] = {ld, ld * a->W, ld * a->W * a->V, ld * a->W * a->V * a->H};
-    const uint32_t box[5] = {64u, (uint32_t)p.qw, 1u, (uint32_t)p.qh, 1u};
+    const uint32_t bw = p.q_rowmajor ? FA_QBOX : p.qw, bh = p.q_rowmajor ? 1 : p.qh;
+    const uint32_t box[5] = {64u, bw, 1u, bh, 1u};
     int rc = cached_tmap_bf16(&p.mapQ, a->q, 5, dims, str, box, 128);
     if (rc != PN_OK) return rc;
     if (FA_D == 80) {
-      const uint32_t boxx[5] = {16u, (uint32_t)p.qw, 1u, (uint32_t)p.qh, 1u};
+      const uint32_t boxx[5] = {16u, bw, 1u, bh, 1u};
       rc = cached_tmap_bf16(&p.mapQx, a->q, 5, dims, str, boxx, 32);
       if (rc != PN_OK) return rc;
     }
@@ -331,10 +404,11 @@ extern "C" int pn_attention(const pn_attn_args* a, int operand_mode, void* strea
       if (rc != PN_OK) return rc;
     }
   }
-  p.tiles_per_group = p.tiles_x * p.tiles_y;
+  p.tiles_per_group = p.q_rowmajor ? (int)((a->H * a->W + 127) / 128) : p.tiles_x * p.tiles_y;
   const long long items = (long long)p.tiles_per_group * a->heads * a->V * a->F;
   PN_REQUIRE(items > 0 && items < (1ll << 31), "pn_attention: too many query tiles");
-  void (*kern)(FaParams) = FA_D == 80 ? attn_fa_kernel<80> : attn_fa_kernel<64>;
+  const int n_idx = (p.kv_rows + 15) / 16 - 1;
+  void (*kern)(FaParams) = FA_D == 80 ? fa_kernels<80>[n_idx] : fa_kernels<64>[n_idx];
   const size_t smem_total = FA_D == 80 ? FaL<80>::TOTAL : FaL<64>::TOTAL;
   {
     const int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem_total);

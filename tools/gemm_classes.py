@@ -1,10 +1,13 @@
-"""Where the wgmma GEMM / implicit-conv time goes, by launch shape, at the benchmark's ε-evaluation.
+"""Where the wgmma GEMM / implicit-conv and the view / text attention time goes, by launch shape, at the benchmark's
+ε-evaluation.
 
 Runs eager ε-evaluations of the full-size model at bench.py's shape (CFG batch 2 x 8 frames, 6 views of 32x56) on ONE
 stream, with CUDA events around every `ops.gemm` call, the way `bench.py::profile_dominant_kernel` does, and groups the
 launches by (M, N, K·taps, epilogue mode). Per class it prints launches, device time, TF/s, algorithmic bytes and the
 roofline lower bound max(FLOP / 989 TF/s, bytes / 3.35 TB/s) (H100 SXM data sheet, dense bf16 and HBM3), naming the
-bound that binds. The card's name, power limit and SM clock are read in the same run.
+bound that binds. Every `ops.attention_view` / `ops.attention_text` call (attn_fa_kernel) is timed the same way and listed
+by kind and shape with its algorithmic TF/s (4 · queries · keys · channels FLOP). The card's name, power limit and SM
+clock are read in the same run.
 
   python tools/gemm_classes.py [--repeats 3] [--json classes.json]
 
@@ -32,11 +35,13 @@ HOST_HEAD_START_CYCLES = 1_000_000_000       # ~0.5 s at 2 GHz, more than the ho
 
 
 def record_launches(ops, run, repeats):
-    """Calls run() `repeats` times with every ops.gemm call timed; returns one list of launch records per repeat."""
+    """Calls run() `repeats` times with every ops.gemm and attention call timed; returns (gemm, attention) launch
+    records, one list per repeat each."""
     # the timing wrapper and its byte count restate bench.py::profile_dominant_kernel (which keeps no shape per launch);
     # keep the two in step
     orig = ops.gemm
-    passes = []
+    orig_view, orig_text = ops.attention_view, ops.attention_text
+    passes, attn = [], []
 
     def timed(a, w, **kw):
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -55,18 +60,59 @@ def record_launches(ops, run, repeats):
         passes[-1].append(((rows, w.shape[0], w.shape[1], mode), 2.0 * rows * w.shape[0] * w.shape[1], abytes, s, e))
         return out
 
-    ops.gemm = timed
+    def timed_view(qkv, heads, cross, neighbours):
+        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        s.record()
+        out = orig_view(qkv, heads, cross, neighbours)
+        e.record()
+        Fr, H, V, w, C3 = qkv.shape
+        keys = sum(len(neighbours[v]) for v in range(V)) if cross else V
+        attn[-1].append((("cross" if cross else "intra", f"{Fr}x{H}x{V}x{w} C={C3 // 3} h={heads}"),
+                         4.0 * Fr * (H * w) ** 2 * keys * (C3 // 3), s, e))
+        return out
+
+    def timed_text(q, kv, heads):
+        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        s.record()
+        out = orig_text(q, kv, heads)
+        e.record()
+        b, Nq, C = q.shape
+        attn[-1].append((("text", f"{b}x{Nq} Nk={kv.shape[1]} C={C} h={heads}"), 4.0 * b * Nq * kv.shape[1] * C, s, e))
+        return out
+
+    ops.gemm, ops.attention_view, ops.attention_text = timed, timed_view, timed_text
     try:
         for _ in range(repeats):
             passes.append([])
+            attn.append([])
             # hold the device back until the host has queued the evaluation: otherwise an event pair around a short
             # launch also spans the host's time to issue it wherever the device has caught up with the host
             torch.cuda._sleep(HOST_HEAD_START_CYCLES)
             run()
             torch.cuda.synchronize()
     finally:
-        ops.gemm = orig
-    return passes
+        ops.gemm, ops.attention_view, ops.attention_text = orig, orig_view, orig_text
+    return passes, attn
+
+
+def classify_attention(attn):
+    per = defaultdict(lambda: {"launches": 0, "flop": 0.0, "secs": []})
+    for i, recs in enumerate(attn):
+        for key, flop, s, e in recs:
+            c = per[key]
+            if i == 0:
+                c["launches"] += 1
+                c["flop"] += flop
+            if len(c["secs"]) <= i:
+                c["secs"].append(0.0)
+            c["secs"][i] += s.elapsed_time(e) * 1e-3
+    rows = []
+    for (kind, shape), c in per.items():
+        secs = statistics.median(c["secs"])
+        rows.append({"kind": kind, "shape": shape, "launches": c["launches"], "ms": secs * 1e3,
+                     "ms_runs": [x * 1e3 for x in c["secs"]], "gflop": c["flop"] / 1e9, "tflops": c["flop"] / secs / 1e12})
+    rows.sort(key=lambda r: -r["ms"])
+    return rows
 
 
 def classify(passes):
@@ -122,7 +168,7 @@ def main():
 
     clocks = bench.ClockSampler(0)
     clocks.start()
-    passes = record_launches(eng.ops, lambda: eng.eps(x_in, concat, t), args.repeats)
+    passes, attn = record_launches(eng.ops, lambda: eng.eps(x_in, concat, t), args.repeats)
     clk = clocks.stop()
     name, limit = card()
 
@@ -144,10 +190,18 @@ def main():
         gf = sum(r["gflop"] for r in sel)
         print(f"  {label:>14}: {sum(r['launches'] for r in sel):4d} launches {gf / 1e3:6.1f} TFLOP {ms:8.1f} ms "
               f"{(gf / ms if ms else 0):6.0f} TF/s")
+    arows = classify_attention(attn)
+    attn_ms = sum(r["ms"] for r in arows)
+    print(f"{len(attn[0])} attention launches (attn_fa_kernel) per ε-evaluation, {attn_ms:.2f} ms, "
+          f"{sum(r['gflop'] for r in arows) / attn_ms if attn_ms else 0:.0f} TF/s")
+    print(f"{'kind':>6} {'shape':>32} {'launch':>6} {'ms':>8} {'TF/s':>6} {'GFLOP':>8}")
+    for r in arows:
+        print(f"{r['kind']:>6} {r['shape']:>32} {r['launches']:>6} {r['ms']:>8.3f} {r['tflops']:>6.0f} {r['gflop']:>8.1f}")
     if args.json:
         Path(args.json).parent.mkdir(parents=True, exist_ok=True)
         Path(args.json).write_text(json.dumps({"card": name, "power_limit": limit, "clocks": clk, "repeats": args.repeats,
-                                               "launches": len(passes[0]), "total_ms": total_ms, "classes": rows}, indent=1))
+                                               "launches": len(passes[0]), "total_ms": total_ms, "classes": rows,
+                                               "attention_ms": attn_ms, "attention": arows}, indent=1))
 
 
 if __name__ == "__main__":

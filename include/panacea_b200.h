@@ -30,6 +30,8 @@
 extern "C" {
 #endif
 
+/* Changes when an existing entry point or struct changes or goes; an added entry point leaves it, since every caller
+ * of the previous surface still links and behaves the same. */
 #define PN_ABI_VERSION 4
 
 enum pn_status { PN_STATUS_OK = 0, PN_STATUS_INVALID = -1, PN_STATUS_CUDA = -2, PN_STATUS_UNSUPPORTED = -3 };
@@ -287,6 +289,25 @@ typedef struct pn_sampler_step_args {
 } pn_sampler_step_args;
 
 int pn_sampler_step(const pn_sampler_step_args* args, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * Layout maps: the ControlNet's 19-channel hint [frames, 19, H, 6w] (fp32, values k/255) of one clip, rendered from
+ * per-panel primitive lists (panacea_b200/layout.py builds them; DESIGN.md section 12). The reference renders the same
+ * channels with OpenCV in its dataset (sgm/data/nuscenes_video/nuscenes_datasets_video.py:286-412).
+ *  prims          [n, PN_LAYOUT_PRIM_FLOATS] fp32, 16-byte aligned, grouped by panel (frame-major, 6 panels per
+ *                 frame). A record is {kind, key, c0, c1, c2, radius, 0, 0, p0.x, p0.y, p1.x, p1.y, p2.x, p2.y, p3.x,
+ *                 p3.y}; a RECT is {kind, class, value, -, -, -, 0, 0, x0, y0, x1, y1, ...} (half-open pixel range).
+ *  panel_offsets  [frames * 6 + 1] int32: the records of panel i are prims[panel_offsets[i] .. panel_offsets[i+1]).
+ *  rays           [6 * 12 + 2] fp64: per panel the first three rows of its img2lidar matrix, then the global min and
+ *                 max of the ray components over all panels.
+ * Channels 0..2 take the colour of the highest-keyed QUAD or BOX_SEGMENT covering a pixel, 13..15 that of the
+ * highest-keyed MAP_SEGMENT, channel 3 + class the minimum value of the RECTs of that class (255 where none).
+ * The output is bitwise the same from call to call. */
+enum pn_layout_kind { PN_LAYOUT_RECT = 0, PN_LAYOUT_QUAD = 1, PN_LAYOUT_BOX_SEGMENT = 2, PN_LAYOUT_MAP_SEGMENT = 3 };
+#define PN_LAYOUT_PRIM_FLOATS 16
+
+int pn_render_layout(const float* prims, const int32_t* panel_offsets, const double* rays, float* out, int64_t frames,
+                     int64_t height, int64_t view_width, void* stream);
 
 #ifdef __cplusplus
 }

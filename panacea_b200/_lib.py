@@ -91,6 +91,7 @@ SIGNATURES: dict[str, tuple] = {
     "pn_scale_dup": (C.c_int, [_vp, _vp, _i64, _f32, C.c_int, _vp]),
     "pn_fingerprint": (C.c_int, [_vp, _i64, _vp, _vp]),
     "pn_softmax_rows_operand": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _f32, C.c_int, _vp]),
+    "pn_render_layout": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp]),
 }
 
 

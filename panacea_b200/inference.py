@@ -3,8 +3,9 @@
 model built from `configs/inference_nuscenes.yaml`-style YAML via instantiate_from_config, `log_images` per batch, frame
 writers. SURVEY.md section 8f rows N1 (engine / conditioner glue) and N3 (writers, gather -> rank-0 writer).
 
-What is NOT here, and why: the nuScenes dataset + BEV rasteriser (row N4, needs nuScenes and mmdet3d) is replaced by
-`SyntheticBEVDataset` with the same batch contract. The VAE (encoder and decoder) is native and random-init unless a
+What is NOT here, and why: the nuScenes dataset itself (needs nuScenes and mmdet3d) is replaced by `SyntheticBEVDataset`
+with the same batch contract, or, with `--layout scene.npz`, by `LayoutDataset`: a scene file of boxes, map polylines and
+cameras whose 19-channel layout maps are rendered on the GPU (panacea_b200/layout.py, DESIGN.md section 12). The VAE (encoder and decoder) is native and random-init unless a
 checkpoint provides `first_stage_model.*`. The OpenCLIP text tower is native too once it has weights: from the checkpoint
 (`conditioner.embedders.0.model.*`) or from a stock open_clip file given as the embedder's `version`; prompts are
 tokenized with the CLIP BPE vocabulary at the embedder's `bpe_path` (else open_clip's bundled copy). Without weights the
@@ -22,15 +23,20 @@ import importlib
 import os
 import time
 
+from pathlib import Path
+
+import numpy as np
 import torch
 import torch.distributed as dist
 import yaml
+from PIL import Image
 from torch.utils.data import DataLoader, Dataset
 from torch.utils.data.distributed import DistributedSampler
 
 from . import dist_utils as D
 from . import frame_io as IO
-from .scene import scene_frame_number
+from . import layout as L
+from .scene import condition_from_frame, scene_frame_number, scene_length
 from .sgm.util import instantiate_from_config
 
 
@@ -73,6 +79,60 @@ class SyntheticBEVDataset(Dataset):
             return first
         return {"clips": [first] + [{"cond_img": torch.rand(self.T, 19, self.h, W, generator=g), "txt": txt,
                                      "filenames": self._names(idx, c)} for c in range(1, self.clips)]}
+
+
+class LayoutDataset(Dataset):
+    """One scene file (panacea_b200/layout.py) as a dataset of one item with the batch contract of `MyDataset` (see
+    `SyntheticBEVDataset`), without the ground-truth `jpg`: `cond_img` rendered on `device` by `render_layout`,
+    `final_cond_zero`, `txt` and `filenames`. The scene must hold K(T-1)+1 frames for K = `clips`; clip k renders the
+    scene frames that `scene.scene_slices` assigns to it, the boundary frame shared with its neighbour. Clip 0 is
+    conditioned on a real frame: `cond_frame` or the scene file's `cond_frame`, an RGB image of [H, 6w] in the
+    panel order of the renderer, which becomes clip 0's frame at the conditioning index. The caption is the file's
+    `prompt`, else one written from the classes of each clip's last frame (the reference captions a clip by its last
+    frame, :541)."""
+
+    def __init__(self, path, num_frames=8, image_hw=(256, 512), use_last_frame=True, clips=1, cond_frame=None,
+                 device="cuda"):
+        if clips < 1:
+            raise ValueError(f"clips must be >= 1, got {clips}")
+        self.path, self.T, (self.h, self.w) = Path(path), num_frames, tuple(image_hw)
+        self.use_last_frame, self.clips, self.device = use_last_frame, clips, device
+        self.scene = L.load_scene(path)
+        want = scene_length(clips, num_frames)
+        if self.scene.num_frames != want:
+            raise L.SceneError(f"{self.path.name}: {self.scene.num_frames} frames, but {clips} clips of {num_frames} "
+                               f"frames need {want}")
+        src = cond_frame or self.scene.cond_frame
+        if src is None:
+            raise L.SceneError(f"{self.path.name}: clip 0 needs a conditioning frame (--cond_frame or 'cond_frame')")
+        img = np.asarray(Image.open(src).convert("RGB"))
+        if img.shape != (self.h, 6 * self.w, 3):
+            raise L.SceneError(f"conditioning frame {src}: expected {6 * self.w} x {self.h}, got {img.shape[1]} x {img.shape[0]}")
+        self.cond_frame = torch.from_numpy(img.astype(np.float32) / 127.5 - 1.0).permute(2, 0, 1).contiguous()
+
+    def __len__(self):
+        return 1
+
+    def frames(self, clip):
+        """Scene frame of each of the clip's T frames."""
+        return [scene_frame_number(clip, f, self.clips, self.T, self.use_last_frame) for f in range(self.T)]
+
+    def _clip(self, clip):
+        frames = self.frames(clip)
+        stem = self.path.stem
+        names = [[f"samples/{cam}/{stem}__{cam}__{f:06d}.jpg" for cam in IO.CAMERA_VIEWS] for f in frames]
+        txt = self.scene.prompt or L.caption(self.scene.labels[frames[-1]])
+        batch = {"cond_img": L.render_layout(self.scene, frames, self.h, self.w, self.device), "txt": txt, "filenames": names}
+        if clip == 0:
+            batch["final_cond_zero"] = condition_from_frame(self.cond_frame, self.T, self.use_last_frame)
+        return batch
+
+    def __getitem__(self, idx):
+        if idx != 0:
+            raise IndexError(idx)
+        if self.clips == 1:
+            return self._clip(0)
+        return {"clips": [self._clip(k) for k in range(self.clips)]}
 
 
 def load_config(paths, overrides=()):
@@ -145,7 +205,9 @@ def get_parser():
     p.add_argument("--bs", type=int, default=1)
     p.add_argument("--dataset", type=str, default=None, help="module:Class of a dataset with the MyDataset batch contract")
     p.add_argument("--num_sequences", type=int, default=2)
-    p.add_argument("--image_hw", type=int, nargs=2, default=(256, 512), help="per-view image size of the synthetic dataset")
+    p.add_argument("--image_hw", type=int, nargs=2, default=(256, 512), help="per-view image size of the synthetic or layout dataset")
+    p.add_argument("--layout", type=str, default=None, help="scene file (.npz) whose layout maps condition the clips (DESIGN.md section 12)")
+    p.add_argument("--cond_frame", type=str, default=None, help="conditioning frame of a --layout scene, an [H, 6w] RGB image")
     p.add_argument("--gather", action="store_true", help="gather decoded frames on rank 0 and let rank 0 write them")
     p.add_argument("--randomize_zero_init", action="store_true", help="re-draw the reference's zero-initialised tails (no checkpoint)")
     p.add_argument("--clips", type=_positive_int, default=1,
@@ -161,13 +223,16 @@ def _positive_int(v) -> int:
 
 
 def make_dataset(opt, config):
-    """`--dataset module:Class` (constructed with `clips=` only for scenes, so a one-clip dataset needs no such keyword)
-    or the synthetic dataset; with --clips K > 1 every item is a scene `{"clips": [K clip batches]}`."""
+    """A `--layout` scene file, `--dataset module:Class` (constructed with `clips=` only for scenes, so a one-clip
+    dataset needs no such keyword) or the synthetic dataset; with --clips K > 1 every item is a scene
+    `{"clips": [K clip batches]}`."""
+    T = config["model"]["params"]["network_config"]["params"].get("num_frames", 8)
+    if opt.layout:
+        return LayoutDataset(opt.layout, T, tuple(opt.image_hw), opt.use_last_frame, opt.clips, cond_frame=opt.cond_frame)
     if opt.dataset:
         mod, cls = opt.dataset.split(":")
         kw = {"clips": opt.clips} if opt.clips > 1 else {}
         return getattr(importlib.import_module(mod), cls)(split=opt.split, use_last_frame=opt.use_last_frame, **kw)
-    T = config["model"]["params"]["network_config"]["params"].get("num_frames", 8)
     return SyntheticBEVDataset(opt.num_sequences, T, tuple(opt.image_hw), opt.use_last_frame, seed=opt.seed, clips=opt.clips)
 
 

@@ -290,6 +290,25 @@ typedef struct pn_sampler_step_args {
 
 int pn_sampler_step(const pn_sampler_step_args* args, void* stream);
 
+/* pn_sampler_step_known — pn_sampler_step with the state blended toward a known latent (editing a recorded clip,
+ * DESIGN.md section 13). After the mode's update and the launch's own noise term, per element:
+ *   kn = sigma != 0 ? known[e] + sigma * xi : known[e]    xi = the Philox normal of (seed, draw, e), as above; the
+ *                                                          product and the sum are each rounded once (no FMA)
+ *   o  = m == 1 ? o : m == 0 ? kn : m * o + (1 - m) * kn   m = mask[frame(e) * plane + e % plane]
+ * with frame(e) = e / (channels * plane): x is [frames, channels, h, W] and the mask [frames, h, W] (plane = h * W)
+ * holds one weight per latent pixel for all its channels. Then out / x and x_in_next are written from the blended o;
+ * hist keeps what the mode writes. `sigma` is the noise level of the state the launch leaves in x. */
+typedef struct pn_sampler_known_args {
+  const float* known;       /* [n] the known latent */
+  const float* mask;        /* [n / channels] weights in [0, 1]: 1 keeps the sampler's value, 0 takes the known one */
+  int64_t plane;            /* h * W latent pixels of one channel of one frame */
+  int32_t channels;         /* latent channels sharing one mask value (n % (channels * plane) == 0) */
+  uint64_t seed, draw;      /* Philox key and draw index of the known region's noise */
+  float sigma;              /* s above */
+} pn_sampler_known_args;
+
+int pn_sampler_step_known(const pn_sampler_step_args* args, const pn_sampler_known_args* known, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Layout maps: the ControlNet's 19-channel hint [frames, 19, H, 6w] (fp32, values k/255) of one clip, rendered from
  * per-panel primitive lists (panacea_b200/layout.py builds them; DESIGN.md section 12). The reference renders the same
@@ -308,6 +327,14 @@ enum pn_layout_kind { PN_LAYOUT_RECT = 0, PN_LAYOUT_QUAD = 1, PN_LAYOUT_BOX_SEGM
 
 int pn_render_layout(const float* prims, const int32_t* panel_offsets, const double* rays, float* out, int64_t frames,
                      int64_t height, int64_t view_width, void* stream);
+
+/* Where two renders of a clip differ, at latent resolution (DESIGN.md section 13). a, b fp32 [frames, 19, H, 6w];
+ * out fp32 [frames, H / cell, 6w / cell] in {0, 1}: 1 where any channel of any pixel of the cell differs between a and
+ * b, or of a cell of the same panel within Chebyshev distance `dilate` (the dilation stops at panel borders). cell is
+ * a power of two <= 32 that divides H and w (8, the VAE factor, for the editing path); (H / cell) * (w / cell) <=
+ * 49152. Two launches (compare and pool, then dilate in place); the output is bitwise the same from call to call. */
+int pn_layout_change_mask(const float* a, const float* b, float* out, int64_t frames, int64_t height, int64_t view_width,
+                          int64_t cell, int64_t dilate, void* stream);
 
 #ifdef __cplusplus
 }

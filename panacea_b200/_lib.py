@@ -57,6 +57,13 @@ class SamplerStepArgs(C.Structure):
     ]
 
 
+class SamplerKnownArgs(C.Structure):
+    _fields_ = [
+        ("known", C.c_void_p), ("mask", C.c_void_p), ("plane", C.c_int64), ("channels", C.c_int32),
+        ("seed", C.c_uint64), ("draw", C.c_uint64), ("sigma", C.c_float),
+    ]
+
+
 _vp, _i64, _i32, _f32 = C.c_void_p, C.c_int64, C.c_int32, C.c_float
 
 # name -> (restype, argtypes); every symbol declared in include/panacea_b200.h must appear here
@@ -88,10 +95,12 @@ SIGNATURES: dict[str, tuple] = {
     "pn_timestep_embedding": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
     "pn_linear_small": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _i64, _i64, _i64, _i64, C.c_int, C.c_int, _vp]),
     "pn_sampler_step": (C.c_int, [C.POINTER(SamplerStepArgs), _vp]),
+    "pn_sampler_step_known": (C.c_int, [C.POINTER(SamplerStepArgs), C.POINTER(SamplerKnownArgs), _vp]),
     "pn_scale_dup": (C.c_int, [_vp, _vp, _i64, _f32, C.c_int, _vp]),
     "pn_fingerprint": (C.c_int, [_vp, _i64, _vp, _vp]),
     "pn_softmax_rows_operand": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _f32, C.c_int, _vp]),
     "pn_render_layout": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "pn_layout_change_mask": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _vp]),
 }
 
 

@@ -147,7 +147,78 @@ __global__ void __launch_bounds__(LAYOUT_THREADS) render_layout_kernel(
   }
 }
 
+// ---------------------------------------------------------------- change mask (DESIGN.md section 13)
+constexpr int MASK_THREADS = 256, MASK_MAX_CELLS = 49152;
+
+// Pass 1: one thread per pixel column of a cell row compares the 19 channels of its `cell` pixels; the `cell` lanes of a
+// cell (cell divides 32, so a cell never straddles two warps) combine their verdicts with one ballot.
+__global__ void __launch_bounds__(MASK_THREADS) change_cells_kernel(const float* __restrict__ a,
+                                                                    const float* __restrict__ b, float* __restrict__ out,
+                                                                    int H, int Wt, int cell) {
+  const int x = blockIdx.x * MASK_THREADS + threadIdx.x, cy = blockIdx.y, frame = blockIdx.z;
+  bool differs = false;
+  if (x < Wt) {
+    const size_t plane = (size_t)H * Wt;
+    const size_t base = (size_t)frame * LAYOUT_CHANNELS * plane + (size_t)cy * cell * Wt + x;
+    for (int c = 0; c < LAYOUT_CHANNELS; ++c)
+      for (int r = 0; r < cell; ++r) {
+        const size_t i = base + c * plane + (size_t)r * Wt;
+        differs |= a[i] != b[i];
+      }
+  }
+  const unsigned votes = __ballot_sync(0xffffffffu, differs);
+  const int lane = threadIdx.x & 31;
+  if (x < Wt && lane % cell == 0) {
+    const unsigned group = cell == 32 ? 0xffffffffu : ((1u << cell) - 1u) << lane;
+    out[((size_t)frame * (H / cell) + cy) * (Wt / cell) + x / cell] = (votes & group) ? 1.f : 0.f;
+  }
+}
+
+// Pass 2: one CTA per panel dilates its cells in place: the panel is read whole into shared memory before any write.
+__global__ void __launch_bounds__(MASK_THREADS) dilate_cells_kernel(float* __restrict__ out, int ch, int cw, int dilate) {
+  __shared__ unsigned char s[MASK_MAX_CELLS];
+  const int frame = blockIdx.x / LAYOUT_VIEWS, view = blockIdx.x % LAYOUT_VIEWS, Wc = LAYOUT_VIEWS * cw;
+  float* o = out + (size_t)frame * ch * Wc + (size_t)view * cw;
+  for (int i = threadIdx.x; i < ch * cw; i += MASK_THREADS) s[i] = o[(size_t)(i / cw) * Wc + i % cw] != 0.f;
+  __syncthreads();
+  for (int i = threadIdx.x; i < ch * cw; i += MASK_THREADS) {
+    const int y = i / cw, x = i % cw;
+    unsigned char v = 0;
+    for (int yy = max(y - dilate, 0); yy <= min(y + dilate, ch - 1) && !v; ++yy)
+      for (int xx = max(x - dilate, 0); xx <= min(x + dilate, cw - 1); ++xx) v |= s[yy * cw + xx];
+    o[(size_t)y * Wc + x] = v ? 1.f : 0.f;
+  }
+}
+
 }  // namespace pn
+
+extern "C" int pn_layout_change_mask(const float* a, const float* b, float* out, int64_t frames, int64_t height,
+                                     int64_t view_width, int64_t cell, int64_t dilate, void* stream_v) {
+  PN_REQUIRE(a && b && out, "pn_layout_change_mask: null pointer");
+  PN_REQUIRE(cell >= 1 && cell <= 32 && (cell & (cell - 1)) == 0, "pn_layout_change_mask: cell %lld is not a power of two <= 32",
+             (long long)cell);
+  PN_REQUIRE(frames > 0 && frames <= 65535 / pn::LAYOUT_VIEWS && height > 0 && view_width > 0 &&
+             height * view_width * pn::LAYOUT_VIEWS <= (int64_t)1 << 31,
+             "pn_layout_change_mask: bad clip size %lld x %lld x %lld", (long long)frames, (long long)height,
+             (long long)view_width);
+  PN_REQUIRE(height % cell == 0 && view_width % cell == 0, "pn_layout_change_mask: %lld x %lld is not a multiple of cell %lld",
+             (long long)height, (long long)view_width, (long long)cell);
+  PN_REQUIRE((height / cell) * (view_width / cell) <= pn::MASK_MAX_CELLS, "pn_layout_change_mask: more than %d cells per panel",
+             pn::MASK_MAX_CELLS);
+  PN_REQUIRE(dilate >= 0, "pn_layout_change_mask: dilate %lld < 0", (long long)dilate);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+  const int64_t Wt = view_width * pn::LAYOUT_VIEWS;
+  const dim3 grid((unsigned)((Wt + pn::MASK_THREADS - 1) / pn::MASK_THREADS), (unsigned)(height / cell), (unsigned)frames);
+  pn::change_cells_kernel<<<grid, pn::MASK_THREADS, 0, st>>>(a, b, out, (int)height, (int)Wt, (int)cell);
+  PN_CHECK_CUDA(cudaGetLastError());
+  if (dilate > 0) {
+    const int d = (int)(dilate < 65536 ? dilate : 65536);     // a panel has fewer cells per side
+    pn::dilate_cells_kernel<<<(unsigned)(frames * pn::LAYOUT_VIEWS), pn::MASK_THREADS, 0, st>>>(
+        out, (int)(height / cell), (int)(view_width / cell), d);
+    PN_CHECK_CUDA(cudaGetLastError());
+  }
+  return pn::PN_OK;
+}
 
 extern "C" int pn_render_layout(const float* prims, const int32_t* panel_offsets, const double* rays, float* out,
                                 int64_t frames, int64_t height, int64_t view_width, void* stream_v) {

@@ -45,8 +45,12 @@ __device__ __forceinline__ float philox_normal(uint64_t seed, uint64_t draw, uin
 }
 
 // ---------------------------------------------------------------- the step kernel
-template <int MODE>
-__global__ void sampler_step_kernel(pn_sampler_step_args a) {
+// KNOWN = false takes an empty second argument, so those instantiations compile to the plain step kernel.
+template <bool KNOWN> struct KnownArgs {};
+template <> struct KnownArgs<true> : pn_sampler_known_args {};
+
+template <int MODE, bool KNOWN>
+__global__ void sampler_step_kernel(pn_sampler_step_args a, KnownArgs<KNOWN> k) {
   const size_t n = (size_t)a.n;
   float* out = a.out ? a.out : a.x;
   for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x) {
@@ -90,6 +94,14 @@ __global__ void sampler_step_kernel(pn_sampler_step_args a) {
       const float xi = a.noise ? a.noise[e] : philox_normal(a.seed, a.draw, e);
       o = o + xi * a.noise_scale * a.noise_amp;
     }
+    if constexpr (KNOWN) {              // blend toward the known latent (pn_sampler_step_known)
+      const float m = k.mask[(e / ((size_t)k.channels * k.plane)) * k.plane + e % k.plane];
+      if (m != 1.f) {
+        float kn = k.known[e];
+        if (k.sigma != 0.f) kn = __fadd_rn(kn, __fmul_rn(k.sigma, philox_normal(k.seed, k.draw, e)));
+        o = m == 0.f ? kn : m * o + (1.f - m) * kn;
+      }
+    }
     out[e] = o;
     if (a.x_in_next) {                  // next network input: x * c_in, duplicated for CFG
       const float v = o * a.c_in_next;
@@ -102,7 +114,8 @@ __global__ void sampler_step_kernel(pn_sampler_step_args a) {
 
 using namespace pn;
 
-extern "C" int pn_sampler_step(const pn_sampler_step_args* a, void* stream_v) {
+template <bool KNOWN>
+static int launch_sampler_step(const pn_sampler_step_args* a, KnownArgs<KNOWN> k, void* stream_v) {
   PN_REQUIRE(a && a->x && a->n > 0, "pn_sampler_step: bad arguments");
   PN_REQUIRE(a->mode >= PN_SAMPLER_EULER && a->mode <= PN_SAMPLER_SCALE, "pn_sampler_step: mode %d", a->mode);
   PN_REQUIRE(a->halves == 1 || a->halves == 2, "pn_sampler_step: halves %d", a->halves);
@@ -117,14 +130,28 @@ extern "C" int pn_sampler_step(const pn_sampler_step_args* a, void* stream_v) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
   const dim3 grid(stride_grid((size_t)a->n)), block(256);
   switch (a->mode) {
-    case PN_SAMPLER_EULER: sampler_step_kernel<PN_SAMPLER_EULER><<<grid, block, 0, st>>>(*a); break;
-    case PN_SAMPLER_HEUN: sampler_step_kernel<PN_SAMPLER_HEUN><<<grid, block, 0, st>>>(*a); break;
-    case PN_SAMPLER_LMS: sampler_step_kernel<PN_SAMPLER_LMS><<<grid, block, 0, st>>>(*a); break;
-    case PN_SAMPLER_DPM: sampler_step_kernel<PN_SAMPLER_DPM><<<grid, block, 0, st>>>(*a); break;
-    case PN_SAMPLER_DPM_2M: sampler_step_kernel<PN_SAMPLER_DPM_2M><<<grid, block, 0, st>>>(*a); break;
-    default: sampler_step_kernel<PN_SAMPLER_SCALE><<<grid, block, 0, st>>>(*a); break;
+    case PN_SAMPLER_EULER: sampler_step_kernel<PN_SAMPLER_EULER, KNOWN><<<grid, block, 0, st>>>(*a, k); break;
+    case PN_SAMPLER_HEUN: sampler_step_kernel<PN_SAMPLER_HEUN, KNOWN><<<grid, block, 0, st>>>(*a, k); break;
+    case PN_SAMPLER_LMS: sampler_step_kernel<PN_SAMPLER_LMS, KNOWN><<<grid, block, 0, st>>>(*a, k); break;
+    case PN_SAMPLER_DPM: sampler_step_kernel<PN_SAMPLER_DPM, KNOWN><<<grid, block, 0, st>>>(*a, k); break;
+    case PN_SAMPLER_DPM_2M: sampler_step_kernel<PN_SAMPLER_DPM_2M, KNOWN><<<grid, block, 0, st>>>(*a, k); break;
+    default: sampler_step_kernel<PN_SAMPLER_SCALE, KNOWN><<<grid, block, 0, st>>>(*a, k); break;
   }
   PN_CHECK_CUDA(cudaGetLastError());
   return PN_OK;
+}
+
+extern "C" int pn_sampler_step(const pn_sampler_step_args* a, void* stream_v) {
+  return launch_sampler_step(a, KnownArgs<false>{}, stream_v);
+}
+
+extern "C" int pn_sampler_step_known(const pn_sampler_step_args* a, const pn_sampler_known_args* k, void* stream_v) {
+  PN_REQUIRE(a && k && k->known && k->mask, "pn_sampler_step_known: bad arguments");
+  PN_REQUIRE(k->channels > 0 && k->plane > 0 && a->n % ((int64_t)k->channels * k->plane) == 0,
+             "pn_sampler_step_known: n = %lld is not a whole number of frames of %d x %lld", (long long)a->n,
+             k->channels, (long long)k->plane);
+  KnownArgs<true> kk;
+  static_cast<pn_sampler_known_args&>(kk) = *k;
+  return launch_sampler_step(a, kk, stream_v);
 }
 

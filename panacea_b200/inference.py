@@ -11,6 +11,8 @@ checkpoint provides `first_stage_model.*`. The OpenCLIP text tower is native too
 tokenized with the CLIP BPE vocabulary at the embedder's `bpe_path` (else open_clip's bundled copy). Without weights the
 embedder is a deterministic stand-in. With the real modules importable, `--dataset module:Class` and the YAML targets
 swap them in. `--clips K` generates scenes of K clips chained through their boundary frame (DESIGN.md section 11).
+`--strength S` edits each item's recorded frames instead of sampling from noise, and with `--layout EDITED.npz
+--mask_from ORIGINAL.npz` regenerates only where the edited layout differs from the original (DESIGN.md section 13).
 Overrides use the dotlist form, and a numeric component indexes a list:
 
   torchrun --nproc-per-node 8 -m panacea_b200.inference --base configs.yaml --name run1 --inferdir out --gather
@@ -36,7 +38,7 @@ from torch.utils.data.distributed import DistributedSampler
 from . import dist_utils as D
 from . import frame_io as IO
 from . import layout as L
-from .scene import condition_from_frame, scene_frame_number, scene_length
+from .scene import cond_index, condition_from_frame, scene_frame_number, scene_length
 from .sgm.util import instantiate_from_config
 
 
@@ -89,26 +91,40 @@ class LayoutDataset(Dataset):
     conditioned on a real frame: `cond_frame` or the scene file's `cond_frame`, an RGB image of [H, 6w] in the
     panel order of the renderer, which becomes clip 0's frame at the conditioning index. The caption is the file's
     `prompt`, else one written from the classes of each clip's last frame (the reference captions a clip by its last
-    frame, :541)."""
+    frame, :541).
+
+    A scene with `frame_files` also gives each clip its recorded frames as `jpg`. With `edit` (one clip only) those are
+    required and clip 0's image condition is the recorded frame at the conditioning index instead of `cond_frame`."""
 
     def __init__(self, path, num_frames=8, image_hw=(256, 512), use_last_frame=True, clips=1, cond_frame=None,
-                 device="cuda"):
+                 device="cuda", edit=False):
         if clips < 1:
             raise ValueError(f"clips must be >= 1, got {clips}")
         self.path, self.T, (self.h, self.w) = Path(path), num_frames, tuple(image_hw)
-        self.use_last_frame, self.clips, self.device = use_last_frame, clips, device
+        self.use_last_frame, self.clips, self.device, self.edit = use_last_frame, clips, device, edit
         self.scene = L.load_scene(path)
         want = scene_length(clips, num_frames)
         if self.scene.num_frames != want:
             raise L.SceneError(f"{self.path.name}: {self.scene.num_frames} frames, but {clips} clips of {num_frames} "
                                f"frames need {want}")
+        if edit:
+            if clips != 1 or cond_frame is not None:
+                raise ValueError("editing takes one clip, conditioned on its own recorded frame")
+            if self.scene.frame_files is None:
+                raise L.SceneError(f"{self.path.name}: editing needs the recorded frames ('frame_files')")
+            self.cond_frame = None
+            return
         src = cond_frame or self.scene.cond_frame
         if src is None:
             raise L.SceneError(f"{self.path.name}: clip 0 needs a conditioning frame (--cond_frame or 'cond_frame')")
+        self.cond_frame = self._read(src, "conditioning frame")
+
+    def _read(self, src, what):
+        """An [H, 6w] RGB image as [3, H, 6w] in [-1, 1]."""
         img = np.asarray(Image.open(src).convert("RGB"))
         if img.shape != (self.h, 6 * self.w, 3):
-            raise L.SceneError(f"conditioning frame {src}: expected {6 * self.w} x {self.h}, got {img.shape[1]} x {img.shape[0]}")
-        self.cond_frame = torch.from_numpy(img.astype(np.float32) / 127.5 - 1.0).permute(2, 0, 1).contiguous()
+            raise L.SceneError(f"{what} {src}: expected {6 * self.w} x {self.h}, got {img.shape[1]} x {img.shape[0]}")
+        return torch.from_numpy(img.astype(np.float32) / 127.5 - 1.0).permute(2, 0, 1).contiguous()
 
     def __len__(self):
         return 1
@@ -123,8 +139,11 @@ class LayoutDataset(Dataset):
         names = [[f"samples/{cam}/{stem}__{cam}__{f:06d}.jpg" for cam in IO.CAMERA_VIEWS] for f in frames]
         txt = self.scene.prompt or L.caption(self.scene.labels[frames[-1]])
         batch = {"cond_img": L.render_layout(self.scene, frames, self.h, self.w, self.device), "txt": txt, "filenames": names}
+        if self.scene.frame_files is not None:
+            batch["jpg"] = torch.stack([self._read(self.scene.frame_files[f], "recorded frame") for f in frames])
         if clip == 0:
-            batch["final_cond_zero"] = condition_from_frame(self.cond_frame, self.T, self.use_last_frame)
+            cond = batch["jpg"][cond_index(self.T, self.use_last_frame)] if self.edit else self.cond_frame
+            batch["final_cond_zero"] = condition_from_frame(cond, self.T, self.use_last_frame)
         return batch
 
     def __getitem__(self, idx):
@@ -212,7 +231,31 @@ def get_parser():
     p.add_argument("--randomize_zero_init", action="store_true", help="re-draw the reference's zero-initialised tails (no checkpoint)")
     p.add_argument("--clips", type=_positive_int, default=1,
                    help="clips per scene: each clip after the first is conditioned on a frame of the one before (DESIGN.md section 11)")
+    p.add_argument("--strength", type=float, default=None,
+                   help="edit each item's recorded frames: re-denoise their latent from this fraction of the schedule, in (0, 1] "
+                        "(DESIGN.md section 13)")
+    p.add_argument("--mask_from", type=str, default=None,
+                   help="original scene file: with --layout EDITED.npz --strength, regenerate only where the layouts differ")
+    p.add_argument("--mask_dilate", type=int, default=1, help="latent cells the --mask_from change mask grows by within a panel")
     return p
+
+
+def check_edit_args(opt):
+    """The editing options that cannot be combined; raises ValueError with the reason."""
+    if opt.strength is not None:
+        if not 0.0 < opt.strength <= 1.0:
+            raise ValueError(f"--strength must lie in (0, 1], got {opt.strength}")
+        if opt.clips > 1:
+            raise ValueError("--strength edits one recorded clip; it cannot be combined with --clips > 1")
+        if opt.cond_frame is not None:
+            raise ValueError("--strength conditions on the clip's own recorded frame; --cond_frame cannot be given with it")
+    if opt.mask_from is not None:
+        if opt.layout is None:
+            raise ValueError("--mask_from compares the --layout scene with the original: it needs --layout EDITED.npz")
+        if opt.strength is None:
+            raise ValueError("--mask_from regenerates part of a recorded clip: it needs --strength")
+    if opt.mask_dilate < 0:
+        raise ValueError(f"--mask_dilate must be >= 0, got {opt.mask_dilate}")
 
 
 def _positive_int(v) -> int:
@@ -228,7 +271,8 @@ def make_dataset(opt, config):
     `{"clips": [K clip batches]}`."""
     T = config["model"]["params"]["network_config"]["params"].get("num_frames", 8)
     if opt.layout:
-        return LayoutDataset(opt.layout, T, tuple(opt.image_hw), opt.use_last_frame, opt.clips, cond_frame=opt.cond_frame)
+        return LayoutDataset(opt.layout, T, tuple(opt.image_hw), opt.use_last_frame, opt.clips, cond_frame=opt.cond_frame,
+                             edit=opt.strength is not None)
     if opt.dataset:
         mod, cls = opt.dataset.split(":")
         kw = {"clips": opt.clips} if opt.clips > 1 else {}
@@ -240,6 +284,7 @@ def main(argv=None):
     opt, unknown = get_parser().parse_known_args(argv)
     if not opt.name:
         raise ValueError("You must specify the experiment name!!")
+    check_edit_args(opt)
     assert opt.bs == 1, "the reference runs batch size 1 (one sequence per rank and step)"
     inferdir = os.path.join(opt.inferdir, opt.name)
     config = load_config(opt.base, unknown)
@@ -257,6 +302,10 @@ def main(argv=None):
     device = torch.device("cuda", local)
 
     dataset = make_dataset(opt, config)
+    mask = None
+    if opt.mask_from:
+        mask = L.change_mask(L.load_scene(opt.mask_from), dataset.scene, dataset.frames(0), tuple(opt.image_hw),
+                             opt.mask_dilate, device)
     sampler = DistributedSampler(dataset, num_replicas=world, rank=rank, shuffle=False)
     loader = DataLoader(dataset, batch_size=opt.bs, sampler=sampler)
 
@@ -282,7 +331,7 @@ def main(argv=None):
             if key not in ("txt", "filenames"):
                 batch[key] = batch[key].to(device)
         with torch.no_grad():
-            outs = model.log_images(batch)
+            outs = model.log_images(batch) if opt.strength is None else model.edit_images(batch, opt.strength, mask)
         filenames = batch["filenames"]
         samples = outs["samples"]
         if opt.gather and world > 1:                           # BASELINE.json configs[2]: NCCL gather of decoded frames

@@ -32,6 +32,10 @@ Scene file keys (arrays; `np.savez`):
   map_points   (sum, 2|3)    the polylines' points in ego metres, concatenated (z = 0 when 2-D)
   prompt       () str        optional caption; without it `caption` writes one from the class counts
   cond_frame   () str        optional path (relative to the file) of the conditioning frame, an [H, 6w] RGB image
+  frame_files  (num_frames,) str  optional paths (relative to the file) of the scene's recorded frames, [H, 6w] RGB
+                             images: the clip that editing starts from (DESIGN.md section 13)
+
+`change_mask` compares two scenes' renders at latent resolution: where an edited scene differs from its original.
 """
 from __future__ import annotations
 
@@ -64,6 +68,7 @@ BOX_LINE_WIDTH = 2                # :525
 MAP_LINE_WIDTH = 4                # :378
 MAP_SAMPLES = 200                 # render.py:52
 HINT_CHANNELS = 19
+LATENT_CELL = 8                   # pixels per latent cell side: the VAE's downsampling factor
 _PRIM = 16                        # PN_LAYOUT_PRIM_FLOATS
 _RECT, _QUAD, _BOX_SEG, _MAP_SEG = 0, 1, 2, 3
 # draw_rect over corners 0..3 and 4..7 (:71-78, 338-339), after the four edges i -> i+4 (:332-336)
@@ -110,6 +115,7 @@ class Scene:
     polylines: list                # per frame [(map class, [k, 3] float64)] in drawing order
     prompt: str | None = None
     cond_frame: Path | None = None
+    frame_files: list | None = None   # per frame, the Path of the recorded [H, 6w] RGB frame
 
 
 def _need(cond, msg):
@@ -188,9 +194,14 @@ def load_scene(path) -> Scene:
                 polylines[mframe[i]].append((int(mlabels[i]), pts[starts[i]:starts[i] + lengths[i]]))
         prompt = str(z["prompt"]) if "prompt" in keys else None
         cond = path.parent / str(z["cond_frame"]) if "cond_frame" in keys else None
+        files = None
+        if "frame_files" in keys:
+            ff = np.asarray(z["frame_files"])
+            _need(ff.shape == (F,) and ff.dtype.kind == "U", f"frame_files: expected {F} paths, got {ff.dtype} {ff.shape}")
+            files = [path.parent / str(f) for f in ff]
     return Scene(F, {c: l2i[i] for i, c in enumerate(cams)},
                  [corners[box_frame == f] for f in range(F)], [labels[box_frame == f] for f in range(F)],
-                 [sorted(p, key=lambda e: e[0]) for p in polylines], prompt, cond)
+                 [sorted(p, key=lambda e: e[0]) for p in polylines], prompt, cond, files)
 
 
 def caption(labels) -> str:
@@ -387,4 +398,22 @@ def render_layout(scene: Scene, frames, H: int, w: int, device="cuda") -> torch.
     lib = _lib.load()
     _lib.check(lib.pn_render_layout(ptr(d_prims), ptr(d_off), ptr(d_rays), ptr(out), len(frames), H, w, stream),
                "pn_render_layout")
+    return out
+
+
+def change_mask(scene_a: Scene, scene_b: Scene, frames, image_hw, dilate: int = 1, device="cuda") -> torch.Tensor:
+    """[T, H/8, 6w/8] fp32 in {0, 1} on `device`: 1 at the latent cells where the layout maps of the two scenes' frames
+    `frames` differ in any channel, dilated by `dilate` cells within each panel (pn_layout_change_mask)."""
+    if scene_a.num_frames != scene_b.num_frames:
+        raise SceneError(f"the scenes hold {scene_a.num_frames} and {scene_b.num_frames} frames; a change mask needs the same count")
+    H, w = image_hw
+    _need(H % LATENT_CELL == 0 and w % LATENT_CELL == 0, f"image size {H} x {w} is not a multiple of {LATENT_CELL}")
+    _need(int(dilate) >= 0, f"dilate must be >= 0, got {dilate}")
+    frames = list(frames)
+    a, b = (render_layout(sc, frames, H, w, device) for sc in (scene_a, scene_b))
+    out = torch.empty(len(frames), H // LATENT_CELL, len(CAMERA_VIEWS) * w // LATENT_CELL, dtype=torch.float32, device=a.device)
+    ptr = lambda t: C.c_void_p(t.data_ptr())
+    stream = C.c_void_p(torch.cuda.current_stream(a.device).cuda_stream) if a.is_cuda else None
+    _lib.check(_lib.load().pn_layout_change_mask(ptr(a), ptr(b), ptr(out), len(frames), H, w, LATENT_CELL, int(dilate), stream),
+               "pn_layout_change_mask")
     return out

@@ -458,11 +458,15 @@ class NativeOps:
 
     def sampler_step(self, mode, x, net=None, *, x_eval=None, out=None, hist=None, noise=None, x_in_next=None, halves=2,
                      net_is_denoised=False, sigma_q=0.0, cfg_scale=1.0, sigma=0.0, dt=0.0, coef=(), hist_read=(),
-                     hist_write=-1, noise_scale=1.0, noise_amp=0.0, seed=0, draw=0, c_in_next=0.0):
+                     hist_write=-1, noise_scale=1.0, noise_amp=0.0, seed=0, draw=0, c_in_next=0.0, known=None, mask=None,
+                     known_seed=0, known_draw=0, known_sigma=0.0):
         """One pn_sampler_step launch (include/panacea_b200.h): the update of `mode` from the network output `net`
         [halves * n] evaluated at `x_eval` (None: x), written to `out` (None: x, in place), plus optional noise
         (`noise` [n], or the in-kernel Philox stream (seed, draw) when None) and the next network input. fp32 in both
-        precision modes. Returns the destination tensor."""
+        precision modes. Returns the destination tensor.
+
+        With `known` (like x, [frames, channels, h, W]) and `mask` [frames, h, W], one pn_sampler_step_known launch: the
+        result is blended toward known + known_sigma * xi (Philox stream (known_seed, known_draw)) where mask < 1."""
         n = x.numel()
         _req(x.dtype == F32 and x.is_contiguous(), "sampler_step: x must be contiguous fp32")
         for name, t, size in (("net", net, halves * n), ("x_eval", x_eval, n), ("out", out, n), ("noise", noise, n),
@@ -484,7 +488,18 @@ class NativeOps:
         for j, v in enumerate(coef):
             a.coef[j] = float(v)
         a.noise_scale, a.noise_amp, a.c_in_next = float(noise_scale), float(noise_amp), float(c_in_next)
-        _lib.check(self.lib.pn_sampler_step(C.byref(a), _stream()), "pn_sampler_step")
+        if known is None and mask is None:
+            _lib.check(self.lib.pn_sampler_step(C.byref(a), _stream()), "pn_sampler_step")
+        else:
+            _req(x.dim() == 4 and known is not None and mask is not None, "sampler_step: known and mask go together, x [F, C, h, W]")
+            _req(known.dtype == F32 and known.is_contiguous() and known.shape == x.shape and known.device == x.device,
+                 "sampler_step: known must be contiguous fp32 shaped like x")
+            _req(mask.dtype == F32 and mask.is_contiguous() and mask.shape == (x.shape[0], *x.shape[2:]) and mask.device == x.device,
+                 f"sampler_step: mask must be contiguous fp32 {(x.shape[0], *x.shape[2:])}")
+            k = _lib.SamplerKnownArgs()
+            k.known, k.mask, k.plane, k.channels = known.data_ptr(), mask.data_ptr(), x.shape[2] * x.shape[3], x.shape[1]
+            k.seed, k.draw, k.sigma = int(known_seed), int(known_draw), float(known_sigma)
+            _lib.check(self.lib.pn_sampler_step_known(C.byref(a), C.byref(k), _stream()), "pn_sampler_step_known")
         self.launches += 1
         return x if out is None else out
 

@@ -76,6 +76,10 @@ class DiffusionEngine3D(nn.Module):
     @torch.no_grad()
     def sample(self, cond, uc=None, batch_size=16, shape=None, randn=None, **kwargs):
         """diffusion.py:233-255. `randn` (optional) replaces the CPU-generator draw for tests."""
+        return self.sampler(BoundDenoiser(self.denoiser, self.model), self._initial_noise(cond, batch_size, shape, randn), cond,
+                            uc=uc)
+
+    def _initial_noise(self, cond, batch_size, shape, randn=None):
         if randn is None:
             randn = torch.randn(batch_size, *shape)                                 # CPU generator, like the reference (:242)
         randn = randn.to(self.device)
@@ -83,13 +87,22 @@ class DiffusionEngine3D(nn.Module):
             last = cond["concat"].to(self.device)[-1]
             randn = randn + last.unsqueeze(0).expand(self.num_frames, *last.shape).repeat(randn.shape[0] // self.num_frames, 1, 1, 1) \
                 * self.share_noise_level
-        return self.sampler(BoundDenoiser(self.denoiser, self.model), randn, cond, uc=uc)
+        return randn
 
     @torch.no_grad()
     def log_images(self, batch, N=8, sample=True, ucg_keys=None, **kwargs):
         """diffusion.py:300-377 for the SD-2.1 branch the config takes (unconditional prompt = ""), without the text/cond
         renderings (log_conditionings draws strings with PIL fonts — not part of the data path)."""
-        log = {}
+        log, c, uc, N, latent_shape, _ = self._log_inputs(batch, N)
+        if sample:
+            samples = self.sample(c, shape=latent_shape, uc=uc, batch_size=N * self.num_frames)
+            log["samples"] = self.decode_first_stage(samples)
+            log["sample_latents"] = samples
+        return log
+
+    def _log_inputs(self, batch, N):
+        """log_images up to the sampler: (log, c, uc, N, latent shape, z = the encoded ground truth or None)."""
+        log, z = {}, None
         if "cond_img" in batch:
             log["cond_img"] = batch["cond_img"].reshape(-1, *batch["cond_img"].shape[2:]).contiguous()
         batch_uc = dict(batch)
@@ -120,10 +133,29 @@ class DiffusionEngine3D(nn.Module):
                     c[k], uc[k] = (y[k][:N * self.num_frames * 4].to(self.device) for y in (c, uc))
                 else:
                     c[k], uc[k] = (y[k][:N].to(self.device) for y in (c, uc))
-        if sample:
-            samples = self.sample(c, shape=latent_shape, uc=uc, batch_size=N * self.num_frames)
-            log["samples"] = self.decode_first_stage(samples)
-            log["sample_latents"] = samples
+        return log, c, uc, N, latent_shape, z
+
+    @torch.no_grad()
+    def edit_images(self, batch, strength, mask=None, N=8):
+        """log_images for a recorded clip (DESIGN.md section 13): the sampler starts from the clip's own latent z0 =
+        encode(batch["jpg"]) noised to the first sigma of the strength's schedule, z0 + sigma_start eps (eps drawn as
+        `sample` draws it), handed over as (z0 + sigma_start eps) / sqrt(1 + sigma_start^2) since the sampler's first
+        launch scales by sqrt(1 + sigma_0^2) (upstream's do_img2img). `mask` [N T, h, w] in [0, 1] (None: no blending)
+        regenerates only where it is > 0: elsewhere every step's result is the known latent z0 noised to its level, and
+        the final latent is z0 where mask = 0. Returns the log_images keys plus "edit_mask"."""
+        if self.input_key not in batch:
+            raise KeyError(f"edit_images needs the recorded frames in batch[{self.input_key!r}]")
+        sigma = float(self.sampler.sigmas(strength=strength)[0])                  # rejects a bad strength first
+        log, c, uc, N, latent_shape, z = self._log_inputs(batch, N)
+        eps = self._initial_noise(c, N * self.num_frames, latent_shape)
+        x = (z + sigma * eps) / (1.0 + sigma ** 2) ** 0.5
+        if mask is not None:
+            mask = mask.to(self.device, torch.float32).reshape(z.shape[0], *z.shape[2:])
+        samples = self.sampler(BoundDenoiser(self.denoiser, self.model), x, c, uc=uc, strength=strength,
+                               known=None if mask is None else z, mask=mask)
+        log["samples"] = self.decode_first_stage(samples)
+        log["sample_latents"] = samples
+        log["edit_mask"] = torch.ones(z.shape[0], *z.shape[2:], device=z.device) if mask is None else mask
         return log
 
     def _image_condition_key(self) -> str:

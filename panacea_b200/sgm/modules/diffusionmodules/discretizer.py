@@ -9,6 +9,18 @@ def generate_roughly_equally_spaced_steps(num_substeps: int, max_step: int) -> n
     return np.linspace(max_step - 1, 0, num_substeps, endpoint=False).astype(int)[::-1]
 
 
+def img2img_sigmas(sigmas: torch.Tensor, strength: float) -> torch.Tensor:
+    """The tail a denoise from `strength` runs over (upstream sgm.inference.helpers.Img2ImgDiscretizationWrapper): of
+    the n + 1 sigmas, trailing 0 included, the last k = int(strength (n + 1)). strength 1 keeps them all."""
+    strength = float(strength)
+    if not 0.0 < strength <= 1.0:
+        raise ValueError(f"strength must lie in (0, 1], got {strength}")
+    k = int(strength * len(sigmas))
+    if k < 2:
+        raise ValueError(f"strength {strength} keeps {k} of {len(sigmas)} sigmas; a denoise needs at least one step (2)")
+    return sigmas[len(sigmas) - k:]
+
+
 class LegacyDDPMDiscretization:
     def __init__(self, linear_start=0.00085, linear_end=0.0120, num_timesteps=1000):
         self.num_timesteps = num_timesteps

@@ -14,7 +14,13 @@ Noise (churn, ancestral): by default a counter-based Philox4x32-10 stream genera
 seed drawn once per sample from torch's default CPU generator (so `torch.manual_seed` makes a run reproducible). It has
 the distribution of the reference's `torch.randn_like`, not its stream. A caller who sets `noise_sampler` (the
 reference's attribute of AncestralSampler; here on every sampler, the EDM churn included) gets one call per draw,
-`noise_sampler(x) -> tensor like x`, and that tensor is used instead."""
+`noise_sampler(x) -> tensor like x`, and that tensor is used instead.
+
+Editing (DESIGN.md section 13): `strength` < 1 runs the tail of the schedule (discretizer.img2img_sigmas), and a
+`known` latent with a `mask` [N, h, W] blends every launch that leaves a sampler step's result in x (the initial scaling
+and each `_Eval.end` launch) toward known + s xi, s the noise level of that result, in the same launch
+(pn_sampler_step_known). The known region's noise is a second Philox stream, its seed drawn once per sample after the
+churn / ancestral seed, one draw index per blended launch."""
 from __future__ import annotations
 
 import math
@@ -23,6 +29,7 @@ import numpy as np
 import torch
 
 from ...util import default, instantiate_from_config
+from .discretizer import img2img_sigmas
 from .sampling_utils import get_ancestral_step, linear_multistep_coeff, to_neg_log_sigma, to_sigma
 
 DEFAULT_GUIDER = {"target": "sgm.modules.diffusionmodules.guiders.IdentityGuider"}
@@ -71,14 +78,15 @@ class BaseDiffusionSampler:
         self.ops = None                     # op set (default panacea_b200.ops.NativeOps)
         self.host_scalars = {}              # the solver scalars of the last schedule (get_ancestral_step, mults, LMS)
 
-    def sigmas(self, num_steps=None):
-        return self.discretization(self.num_steps if num_steps is None else num_steps, device="cpu")
+    def sigmas(self, num_steps=None, strength=1.0):
+        """The schedule one sample runs over: the discretization's n + 1 sigmas, cut to the tail of `strength`."""
+        return img2img_sigmas(self.discretization(self.num_steps if num_steps is None else num_steps, device="cpu"), strength)
 
     # ------------------------------------------------------------------ host plan
-    def plan(self, num_steps=None):
+    def plan(self, num_steps=None, strength=1.0):
         """(init, evals) for one sample: `init` the keyword scalars of the launch that applies prepare_sampling_loop's
         x *= sqrt(1 + sigma_0^2) (sampling.py:50), `evals` one _Eval per network evaluation."""
-        sig = self.sigmas(num_steps).to(F32)
+        sig = self.sigmas(num_steps, strength).to(F32)
         self.host_scalars = {"ancestral": [], "mult": [], "lms": []}
         init = {"coef": (math.sqrt(1.0 + float(sig[0]) ** 2.0),)}
         return init, self._plan(sig, init)
@@ -91,22 +99,26 @@ class BaseDiffusionSampler:
 
     # ------------------------------------------------------------------ loop
     @torch.no_grad()
-    def __call__(self, denoiser, x, cond, uc=None, num_steps=None):
+    def __call__(self, denoiser, x, cond, uc=None, num_steps=None, *, strength=1.0, known=None, mask=None):
         """x [N,4,H,W] initial noise (unit variance); cond / uc dicts as produced by the conditioner. `denoiser` is any
         callable (x, sigma, cond) -> denoised, like the reference's lambda (diffusion.py:251-254); a `BoundDenoiser`
-        takes the fused path. Returns the final latent, like the reference."""
+        takes the fused path. Returns the final latent, like the reference.
+
+        `strength` in (0, 1] runs the last int(strength (n + 1)) sigmas only (x is then the scaled noisy latent of
+        upstream's do_img2img); `known` [N,4,H,W] with `mask` [N,H,W] in [0, 1] keeps known + sigma xi where mask = 0."""
         if self.ops is None:
             from ....ops import NativeOps
             self.ops = NativeOps()
         uc = default(uc, cond)
-        init, evals = self.plan(num_steps)
+        init, evals = self.plan(num_steps, strength)
+        blend = self._blend_source(x, known, mask, evals)
         if not isinstance(denoiser, BoundDenoiser):
-            return self._generic_loop(denoiser, x, cond, uc, init, evals)
+            return self._generic_loop(denoiser, x, cond, uc, init, evals, blend)
         net = denoiser.network
         cc = self.guider.prepare_cond(cond, uc)                   # once per sample
         if hasattr(net, "prepare"):
             net.prepare(cc)                                       # step-invariant conditioning work, once per sample
-        return self._fused_loop(denoiser.denoiser, net, x, cc, init, evals)
+        return self._fused_loop(denoiser.denoiser, net, x, cc, init, evals, blend)
 
     def _halves(self):
         return 1 if type(self.guider).__name__.startswith("Identity") else 2
@@ -137,7 +149,35 @@ class BaseDiffusionSampler:
             return kw
         return draw
 
-    def _fused_loop(self, den, net, x, cc, init, evals):
+    def _blend_source(self, x, known, mask, evals):
+        """-> blend(k, kw) adding the known-latent arguments of a launch: k = -1 the initial scaling, else the index of
+        the evaluation the launch follows. Only launches that leave a step's result in x blend; s is the sigma the
+        next step's first evaluation sees (its sigma_hat under EDM churn), 0 after the last step."""
+        if known is None and mask is None:
+            return lambda k, kw: kw
+        if known is None or mask is None:
+            raise ValueError("known and mask go together")
+        want = (x.shape[0], *x.shape[2:])
+        if known.shape != x.shape or mask.shape != want:
+            raise ValueError(f"known must be shaped like x {tuple(x.shape)} and mask {want}; got {tuple(known.shape)}, {tuple(mask.shape)}")
+        known = known.to(device=x.device, dtype=F32).contiguous()
+        mask = mask.to(device=x.device, dtype=F32).contiguous()
+        if not (torch.isfinite(mask).all() and ((mask >= 0) & (mask <= 1)).all() and torch.isfinite(known).all()):
+            raise ValueError("mask must be finite and in [0, 1], known finite")
+        level = [e.sigma for e in evals] + [0.0]                   # level[k + 1]: what the launch after eval k leaves
+        state = {"draw": 0}
+
+        def blend(k, kw):
+            if k >= 0 and not evals[k].end:
+                return kw
+            if "seed" not in state:                                # drawn at the first launch, after the churn seed
+                state["seed"] = int(torch.randint(0, 2 ** 62, (1,)).item())
+            kw = dict(kw, known=known, mask=mask, known_seed=state["seed"], known_draw=state["draw"], known_sigma=level[k + 1])
+            state["draw"] += 1
+            return kw
+        return blend
+
+    def _fused_loop(self, den, net, x, cc, init, evals, blend=lambda k, kw: kw):
         ops, halves = self.ops, self._halves()
         n = x.shape[0]
         scal = [den.step_scalars(e.sigma) for e in evals]           # (timestep index, quantised sigma, c_in)
@@ -148,7 +188,7 @@ class BaseDiffusionSampler:
         x_in = torch.empty((halves * n, *x0.shape[1:]), dtype=F32, device=x0.device)
         draw = self._noise_source(init, evals)
         scale = float(getattr(self.guider, "scale", 1.0)) if halves == 2 else 1.0
-        ops.sampler_step(SCALE, x0, out=xs, halves=halves, x_in_next=x_in, c_in_next=scal[0][2], **draw(x0, init))
+        ops.sampler_step(SCALE, x0, out=xs, halves=halves, x_in_next=x_in, c_in_next=scal[0][2], **blend(-1, draw(x0, init)))
         x = xs
         static = hasattr(net, "static_io")
         for k, e in enumerate(evals):
@@ -157,12 +197,12 @@ class BaseDiffusionSampler:
             ops.sampler_step(e.mode, x, eps.float().contiguous(), x_eval=stage if e.at_stage else None,
                              out=stage if e.out_stage else None, hist=hist, x_in_next=None if last else x_in,
                              halves=halves, sigma_q=scal[k][1], cfg_scale=scale, c_in_next=0.0 if last else scal[k + 1][2],
-                             **draw(x, e.kw))
+                             **blend(k, draw(x, e.kw)))
             if e.end and self.step_callback is not None:
                 self.step_callback(e.step, x)
         return x
 
-    def _generic_loop(self, denoiser, x, cond, uc, init, evals):
+    def _generic_loop(self, denoiser, x, cond, uc, init, evals, blend=lambda k, kw: kw):
         """The reference's call contract: an opaque `denoiser(x2, sigma2, cond2) -> denoised2` per evaluation with the
         guider's inputs; guidance combine + solver update in one kernel (net_is_denoised)."""
         ops, halves = self.ops, self._halves()
@@ -171,14 +211,14 @@ class BaseDiffusionSampler:
         x0, xs, stage, hist = self._buffers(x, evals)
         draw = self._noise_source(init, evals)
         scale = float(getattr(self.guider, "scale", 1.0)) if halves == 2 else 1.0
-        ops.sampler_step(SCALE, x0, out=xs, halves=halves, **draw(x0, init))
+        ops.sampler_step(SCALE, x0, out=xs, halves=halves, **blend(-1, draw(x0, init)))
         x = xs
-        for e in evals:
+        for k, e in enumerate(evals):
             s_in = torch.full((n,), e.sigma, dtype=F32, device=x.device)
             x2, s2, c2 = self.guider.prepare_inputs(stage if e.at_stage else x, s_in, cond, uc)
             den2 = denoiser(x2, s2, c2).float().contiguous()
             ops.sampler_step(e.mode, x, den2, x_eval=stage if e.at_stage else None, out=stage if e.out_stage else None,
-                             hist=hist, halves=halves, net_is_denoised=True, cfg_scale=scale, **draw(x, e.kw))
+                             hist=hist, halves=halves, net_is_denoised=True, cfg_scale=scale, **blend(k, draw(x, e.kw)))
             if e.end and self.step_callback is not None:
                 self.step_callback(e.step, x)
         return x

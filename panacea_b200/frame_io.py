@@ -65,9 +65,10 @@ def logs_all_images(outs: dict, root: str, filenames) -> list[str]:
 
 
 def logs_scene(frames: torch.Tensor, inferdir: str, filenames) -> list[str]:
-    """A scene of K chained clips (panacea_b200/scene.py): frames [K(T-1)+1, 3, H, 6*w] and their `filenames`, both in
-    chronological order. Writes `fake/<scene>_<cam>/_{frame:06}.jpg` numbered over the whole scene (the directory named,
-    as for one clip, after the last frame), one PNG strip under `allimages/samples/` and one GIF under `gifs/samples/`."""
+    """A scene of K chained clips sharing m frames (panacea_b200/scene.py): frames [K(T-m)+m, 3, H, 6*w] and their
+    `filenames`, both in chronological order. Writes `fake/<scene>_<cam>/_{frame:06}.jpg` numbered `_000000` ..
+    `_{K(T-m)+m-1:06}` over the whole scene (the directory named, as for one clip, after the last frame), one PNG strip
+    under `allimages/samples/` and one GIF under `gifs/samples/`."""
     outs = {"samples": frames}
     return (logs_frames(frames, os.path.join(inferdir, "fake"), filenames)
             + logs_all_images(outs, os.path.join(inferdir, "allimages"), filenames)

@@ -10,7 +10,8 @@ checkpoint provides `first_stage_model.*`. The OpenCLIP text tower is native too
 (`conditioner.embedders.0.model.*`) or from a stock open_clip file given as the embedder's `version`; prompts are
 tokenized with the CLIP BPE vocabulary at the embedder's `bpe_path` (else open_clip's bundled copy). Without weights the
 embedder is a deterministic stand-in. With the real modules importable, `--dataset module:Class` and the YAML targets
-swap them in. `--clips K` generates scenes of K clips chained through their boundary frame (DESIGN.md section 11).
+swap them in. `--clips K` generates scenes of K clips chained through their boundary frame, and `--overlap M` chains
+them through M shared frames whose latents each clip keeps from the one before (DESIGN.md section 11).
 `--strength S` edits each item's recorded frames instead of sampling from noise, and with `--layout EDITED.npz
 --mask_from ORIGINAL.npz` regenerates only where the edited layout differs from the original (DESIGN.md section 13).
 Overrides use the dotlist form, and a numeric component indexes a list:
@@ -38,7 +39,7 @@ from torch.utils.data.distributed import DistributedSampler
 from . import dist_utils as D
 from . import frame_io as IO
 from . import layout as L
-from .scene import cond_index, condition_from_frame, scene_frame_number, scene_length
+from .scene import check_overlap, cond_index, condition_from_frame, scene_frame_number, scene_length
 from .sgm.util import instantiate_from_config
 
 
@@ -50,20 +51,23 @@ class SyntheticBEVDataset(Dataset):
 
     Scene form (`clips` = K > 1, DESIGN.md section 11): an item is `{"clips": [clip_0, ..., clip_{K-1}]}`. Clip 0 is the
     batch above; clips k > 0 carry only their layout, `cond_img`, `txt` and `filenames`, because their image condition
-    is a frame that clip k-1 generates. A boundary frame has the same file name in both clips that hold it."""
+    is a frame that clip k-1 generates. A frame two clips share (the boundary frame, or the `overlap` shared frames)
+    has the same file name in both clips that hold it."""
 
-    def __init__(self, num_sequences=2, num_frames=8, image_hw=(256, 512), use_last_frame=True, seed=0, clips=1):
+    def __init__(self, num_sequences=2, num_frames=8, image_hw=(256, 512), use_last_frame=True, seed=0, clips=1,
+                 overlap=None):
         self.n, self.T, (self.h, self.w), self.use_last_frame, self.seed = num_sequences, num_frames, image_hw, use_last_frame, seed
         if clips < 1:
             raise ValueError(f"clips must be >= 1, got {clips}")
-        self.clips = clips
+        check_overlap(overlap, num_frames)
+        self.clips, self.overlap = clips, overlap
 
     def __len__(self):
         return self.n
 
     def _names(self, idx, clip):
         scene = f"n015-2018-07-24-11-22-45+0800__seq{idx:04d}"
-        stamp = lambda f: 1532402927 + 50 * scene_frame_number(clip, f, self.clips, self.T, self.use_last_frame)
+        stamp = lambda f: 1532402927 + 50 * scene_frame_number(clip, f, self.clips, self.T, self.use_last_frame, self.overlap)
         return [[f"samples/{cam}/{scene}__{cam}__{stamp(f):d}.jpg" for cam in sorted(IO.VIEW_ID, key=IO.VIEW_ID.get)]
                 for f in range(self.T)]
 
@@ -86,8 +90,9 @@ class SyntheticBEVDataset(Dataset):
 class LayoutDataset(Dataset):
     """One scene file (panacea_b200/layout.py) as a dataset of one item with the batch contract of `MyDataset` (see
     `SyntheticBEVDataset`), without the ground-truth `jpg`: `cond_img` rendered on `device` by `render_layout`,
-    `final_cond_zero`, `txt` and `filenames`. The scene must hold K(T-1)+1 frames for K = `clips`; clip k renders the
-    scene frames that `scene.scene_slices` assigns to it, the boundary frame shared with its neighbour. Clip 0 is
+    `final_cond_zero`, `txt` and `filenames`. The scene must hold K(T-m)+m frames for K = `clips` and m = `overlap`
+    shared frames (1 when None); clip k renders the scene frames that `scene.scene_frame_number` assigns to it, so the
+    frames it shares with its neighbour render from the same scene frames. Clip 0 is
     conditioned on a real frame: `cond_frame` or the scene file's `cond_frame`, an RGB image of [H, 6w] in the
     panel order of the renderer, which becomes clip 0's frame at the conditioning index. The caption is the file's
     `prompt`, else one written from the classes of each clip's last frame (the reference captions a clip by its last
@@ -97,16 +102,18 @@ class LayoutDataset(Dataset):
     required and clip 0's image condition is the recorded frame at the conditioning index instead of `cond_frame`."""
 
     def __init__(self, path, num_frames=8, image_hw=(256, 512), use_last_frame=True, clips=1, cond_frame=None,
-                 device="cuda", edit=False):
+                 device="cuda", edit=False, overlap=None):
         if clips < 1:
             raise ValueError(f"clips must be >= 1, got {clips}")
+        check_overlap(overlap, num_frames)
         self.path, self.T, (self.h, self.w) = Path(path), num_frames, tuple(image_hw)
-        self.use_last_frame, self.clips, self.device, self.edit = use_last_frame, clips, device, edit
+        self.use_last_frame, self.clips, self.device, self.edit, self.overlap = use_last_frame, clips, device, edit, overlap
         self.scene = L.load_scene(path)
-        want = scene_length(clips, num_frames)
+        want = scene_length(clips, num_frames, overlap)
         if self.scene.num_frames != want:
+            shared = "" if overlap is None else f" with {overlap} shared between neighbours"
             raise L.SceneError(f"{self.path.name}: {self.scene.num_frames} frames, but {clips} clips of {num_frames} "
-                               f"frames need {want}")
+                               f"frames{shared} need {want}")
         if edit:
             if clips != 1 or cond_frame is not None:
                 raise ValueError("editing takes one clip, conditioned on its own recorded frame")
@@ -131,7 +138,7 @@ class LayoutDataset(Dataset):
 
     def frames(self, clip):
         """Scene frame of each of the clip's T frames."""
-        return [scene_frame_number(clip, f, self.clips, self.T, self.use_last_frame) for f in range(self.T)]
+        return [scene_frame_number(clip, f, self.clips, self.T, self.use_last_frame, self.overlap) for f in range(self.T)]
 
     def _clip(self, clip):
         frames = self.frames(clip)
@@ -231,6 +238,9 @@ def get_parser():
     p.add_argument("--randomize_zero_init", action="store_true", help="re-draw the reference's zero-initialised tails (no checkpoint)")
     p.add_argument("--clips", type=_positive_int, default=1,
                    help="clips per scene: each clip after the first is conditioned on a frame of the one before (DESIGN.md section 11)")
+    p.add_argument("--overlap", type=int, default=None,
+                   help="frames consecutive clips of a scene share: each clip keeps the previous clip's latents for them and "
+                        "generates the rest; needs --clips >= 2 and 1 <= M <= T-1 (DESIGN.md section 11)")
     p.add_argument("--strength", type=float, default=None,
                    help="edit each item's recorded frames: re-denoise their latent from this fraction of the schedule, in (0, 1] "
                         "(DESIGN.md section 13)")
@@ -258,6 +268,18 @@ def check_edit_args(opt):
         raise ValueError(f"--mask_dilate must be >= 0, got {opt.mask_dilate}")
 
 
+def check_scene_args(opt, num_frames: int):
+    """The scene options that cannot work with clips of `num_frames` frames; raises ValueError with the reason."""
+    if opt.overlap is not None:
+        if opt.clips < 2:
+            raise ValueError(f"--overlap shares frames between consecutive clips: it needs --clips >= 2, got {opt.clips}")
+        check_overlap(opt.overlap, num_frames)
+
+
+def num_frames(config) -> int:
+    return config["model"]["params"]["network_config"]["params"].get("num_frames", 8)
+
+
 def _positive_int(v) -> int:
     n = int(v)
     if n < 1:
@@ -266,18 +288,21 @@ def _positive_int(v) -> int:
 
 
 def make_dataset(opt, config):
-    """A `--layout` scene file, `--dataset module:Class` (constructed with `clips=` only for scenes, so a one-clip
-    dataset needs no such keyword) or the synthetic dataset; with --clips K > 1 every item is a scene
-    `{"clips": [K clip batches]}`."""
-    T = config["model"]["params"]["network_config"]["params"].get("num_frames", 8)
+    """A `--layout` scene file, `--dataset module:Class` (constructed with `clips=` only for scenes and `overlap=` only
+    when --overlap is given, so a one-clip dataset needs no such keyword) or the synthetic dataset; with --clips K > 1
+    every item is a scene `{"clips": [K clip batches]}`."""
+    T = num_frames(config)
     if opt.layout:
         return LayoutDataset(opt.layout, T, tuple(opt.image_hw), opt.use_last_frame, opt.clips, cond_frame=opt.cond_frame,
-                             edit=opt.strength is not None)
+                             edit=opt.strength is not None, overlap=opt.overlap)
     if opt.dataset:
         mod, cls = opt.dataset.split(":")
         kw = {"clips": opt.clips} if opt.clips > 1 else {}
+        if opt.overlap is not None:
+            kw["overlap"] = opt.overlap
         return getattr(importlib.import_module(mod), cls)(split=opt.split, use_last_frame=opt.use_last_frame, **kw)
-    return SyntheticBEVDataset(opt.num_sequences, T, tuple(opt.image_hw), opt.use_last_frame, seed=opt.seed, clips=opt.clips)
+    return SyntheticBEVDataset(opt.num_sequences, T, tuple(opt.image_hw), opt.use_last_frame, seed=opt.seed, clips=opt.clips,
+                               overlap=opt.overlap)
 
 
 def main(argv=None):
@@ -288,6 +313,7 @@ def main(argv=None):
     assert opt.bs == 1, "the reference runs batch size 1 (one sequence per rank and step)"
     inferdir = os.path.join(opt.inferdir, opt.name)
     config = load_config(opt.base, unknown)
+    check_scene_args(opt, num_frames(config))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world > 1:
         local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -355,13 +381,13 @@ def main(argv=None):
 
 
 def _run_scene(model, item, opt, inferdir, rank, world, device) -> list[str]:
-    """One scene of `opt.clips` clips (`DiffusionEngine3D.sample_scene`), written as one chronological sequence per
-    camera plus one PNG strip and one GIF; `--gather` gathers one scene per rank on rank 0."""
+    """One scene of `opt.clips` clips (`DiffusionEngine3D.sample_scene`, sharing `opt.overlap` frames), written as one
+    chronological sequence per camera plus one PNG strip and one GIF; `--gather` gathers one scene per rank on rank 0."""
     clips = item["clips"]
     if len(clips) != opt.clips:
         raise ValueError(f"--clips {opt.clips}, but the dataset item holds {len(clips)} clips")
     with torch.no_grad():
-        out = model.sample_scene(clips, use_last_frame=opt.use_last_frame)
+        out = model.sample_scene(clips, use_last_frame=opt.use_last_frame, overlap=opt.overlap)
     frames, names = out["samples"], out["filenames"]
     if opt.gather and world > 1:
         gathered = D.gather_on_rank0(frames.to(device).contiguous())

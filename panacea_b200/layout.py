@@ -19,7 +19,7 @@ The reference draws the map lines with cv2.LINE_AA on a float64 canvas, where Op
 channel is a plain overwrite.
 
 Scene file keys (arrays; `np.savez`):
-  num_frames   ()            frames in the scene; a scene of K clips of T frames has K(T-1)+1
+  num_frames   ()            frames in the scene; a scene of K clips of T frames sharing m has K(T-m)+m (m = 1 default)
   cameras      (6,) str      the camera of each row of lidar2img (any order, each of CAMERA_VIEWS once)
   lidar2img    (6, 4, 4)     ego -> image, held in fp32 as the reference's dataset holds it
   box_frame    (M,) int      frame of each box

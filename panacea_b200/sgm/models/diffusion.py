@@ -165,25 +165,50 @@ class DiffusionEngine3D(nn.Module):
         return keys[0]
 
     @torch.no_grad()
-    def sample_scene(self, batches, use_last_frame=True, **kwargs):
-        """A scene of K = len(batches) clips chained through their boundary frame (panacea_b200/scene.py).
+    def outpaint_images(self, batch, known, mask, N=8, **kwargs):
+        """log_images with part of the clip given (DESIGN.md section 11): the conditioning, the initial noise and the
+        full-strength schedule of `log_images`, with `known` [N T, 4, h, w] kept where `mask` [N T, h, w] is 0 (the
+        sampler blends every step's result toward known + sigma xi there, so the final latent is `known` exactly) and
+        generated where it is 1. The known region's Philox seed is drawn from the CPU generator after the churn seed.
+        Other `log_images` keywords are accepted and ignored, as `log_images` ignores its own."""
+        log, c, uc, N, latent_shape, _ = self._log_inputs(batch, N)
+        x = self._initial_noise(c, N * self.num_frames, latent_shape)
+        samples = self.sampler(BoundDenoiser(self.denoiser, self.model), x, c, uc=uc, known=known, mask=mask)
+        log["samples"] = self.decode_first_stage(samples)
+        log["sample_latents"] = samples
+        return log
+
+    @torch.no_grad()
+    def sample_scene(self, batches, use_last_frame=True, overlap=None, **kwargs):
+        """A scene of K = len(batches) clips chained through their boundary frame, or through `overlap` = m shared
+        frames (panacea_b200/scene.py).
 
         `batches[k]` is clip k's layout batch as `MyDataset.__getitem__` + the DataLoader give it (one sequence):
         `cond_img`, `txt`, `filenames`; clip 0 also carries the ground truth and its real image condition. Tensors may
         stay on the host: each clip's are moved to the device when that clip runs. Clip k > 0 is
-        conditioned on the frame of clip k-1 at index T-1-a (a = T-1 with `use_last_frame`, else 0), quantised like the
-        writers and read back like the dataset, in a `final_cond_zero` that is zero elsewhere; it goes through the
-        conditioner and the VAE embedder unchanged. Each clip is one `log_images` call, in clip order, so the CPU
-        generator is drawn as K successive calls draw it, and K = 1 is exactly `log_images`. The wrapper replays the
-        one CUDA graph of clip 0 (the conditioning is re-prepared into the same buffers). A clip's decoded frames move
-        to the host before the next clip starts, so the device peak of a scene is that of one clip.
+        conditioned on the frame of clip k-1 that lands on its conditioning index a (a = T-1 with `use_last_frame`,
+        else 0; `scene.handoff_index`), quantised like the writers and read back like the dataset, in a
+        `final_cond_zero` that is zero elsewhere; it goes through the conditioner and the VAE embedder unchanged.
 
-        Returns a dict (all tensors on the host): "samples" the scene [K(T-1)+1, 3, H, W] in chronological order,
-        "sample_latents" the K per-clip latents [T, 4, h, w], "handoff_frames" the K-1 dequantised frames [3, H, W]
-        that conditioned clips 1..K-1, "clip_samples" the K decoded clips [T, 3, H, W], and "filenames" in scene order
-        when the batches carry them."""
+        `overlap` None: each clip is one `log_images` call, in clip order, so the CPU generator is drawn as K successive
+        calls draw it, and K = 1 is exactly `log_images`; clip k > 0 regenerates the boundary frame and the scene keeps
+        clip k-1's copy. `overlap` m in 1 .. T-1: clip 0 is one `log_images` call and clip k > 0 one `outpaint_images`
+        call, which keeps clip k-1's final latents of the m shared frames (`scene.known_region`) and generates the other
+        T-m; the shared latents, and so their decoded frames, come out equal to clip k-1's. Per carrying clip the CPU
+        generator gives the initial noise, then the churn seed (noisy samplers only), then the known region's seed, as
+        `edit_images` draws them; so the draws of clips k > 1 differ from the same scene with `overlap` None.
+
+        The wrapper replays the one CUDA graph of clip 0 (the conditioning is re-prepared into the same buffers). A
+        clip's decoded frames and latent move to the host before the next clip starts, and the latent comes back to
+        the device only as the next clip's known region, so the device peak of a scene is that of one clip.
+
+        Returns a dict (all tensors on the host): "samples" the scene [K(T-m)+m, 3, H, W] in chronological order (m = 1
+        for `overlap` None), "sample_latents" the K per-clip latents [T, 4, h, w], "handoff_frames" the K-1 dequantised
+        frames [3, H, W] that conditioned clips 1..K-1, "clip_samples" the K decoded clips [T, 3, H, W], "overlap", and
+        "filenames" in scene order when the batches carry them."""
         from ... import scene as S
         T = self.num_frames
+        S.check_overlap(overlap, T)
         key = self._image_condition_key() if len(batches) > 1 else None
         clips, latents, handoffs = [], [], []
         for k, batch in enumerate(batches):
@@ -192,16 +217,21 @@ class DiffusionEngine3D(nn.Module):
                 cond = S.condition_from_frame(handoffs[-1], T, use_last_frame)
                 batch = {n: v for n, v in batch.items() if n != self.input_key}
                 batch[key] = cond.unsqueeze(0).to(self.device)
-            log = self.log_images(batch, **kwargs)
+            if k > 0 and overlap is not None:
+                known, mask = S.known_region(latents[-1].to(self.device), use_last_frame, overlap)
+                log = self.outpaint_images(batch, known, mask, **kwargs)
+                del known, mask
+            else:
+                log = self.log_images(batch, **kwargs)
             if log["samples"].shape[0] != T:
                 raise ValueError(f"a scene clip is one sequence of {T} frames; clip {k} decoded {log['samples'].shape[0]}")
             clips.append(log["samples"].cpu())
             latents.append(log["sample_latents"].cpu())
             del log                                                         # the clip's device tensors go before the next clip
             if k + 1 < len(batches):
-                handoffs.append(S.quantize_frame(clips[-1][S.handoff_index(T, use_last_frame)]))
-        out = {"samples": S.scene_order(clips, use_last_frame), "sample_latents": latents, "handoff_frames": handoffs,
-               "clip_samples": clips}
+                handoffs.append(S.quantize_frame(clips[-1][S.handoff_index(T, use_last_frame, overlap)]))
+        out = {"samples": S.scene_order(clips, use_last_frame, overlap), "sample_latents": latents,
+               "handoff_frames": handoffs, "clip_samples": clips, "overlap": overlap}
         if all("filenames" in b for b in batches):
-            out["filenames"] = S.scene_order([b["filenames"] for b in batches], use_last_frame)
+            out["filenames"] = S.scene_order([b["filenames"] for b in batches], use_last_frame, overlap)
         return out

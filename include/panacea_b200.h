@@ -336,6 +336,26 @@ int pn_render_layout(const float* prims, const int32_t* panel_offsets, const dou
 int pn_layout_change_mask(const float* a, const float* b, float* out, int64_t frames, int64_t height, int64_t view_width,
                           int64_t cell, int64_t dilate, void* stream);
 
+/* A user-drawn edit mask at latent resolution (DESIGN.md section 13). pixels uint8 [frames, H, 6w], nonzero = regenerate;
+ * out fp32 [frames, H / cell, 6w / cell] in {0, 1}: 1 where any pixel of the cell is nonzero, dilated by `dilate` cells
+ * within each panel exactly as pn_layout_change_mask dilates. Same limits as pn_layout_change_mask. */
+int pn_mask_cells(const uint8_t* pixels, float* out, int64_t frames, int64_t height, int64_t view_width, int64_t cell,
+                  int64_t dilate, void* stream);
+
+/* Paste the recorded pixels back outside an edit (DESIGN.md section 13). decoded, recorded, out fp32 [frames, 3, H, 6w];
+ * cells fp32 [frames, H / cell, 6w / cell], a cell > 0 is regenerated; alpha fp32 [frames, H, 6w] or NULL. For pixel
+ * (y, x) of panel v, with R the regenerated cells of the same frame and panel (nothing crosses a panel seam):
+ *   d2    = min over c in R of dx^2 + dy^2, dx = max(0, c.x0 - x, x - c.x1) (c.x0, c.x1 its first and last pixel
+ *           column; dy likewise with rows): the squared distance between pixel centres, an integer;
+ *   alpha = 1 if d2 = 0; 0 if R is empty; else max(0, 1 - sqrt(d2) / (feather + 1)), each operation IEEE fp32;
+ *   b     = clamp(rint((recorded + 1) * 127.5), 0, 255), k = (b + 0.5) / 127.5 - 1 (fp32): the recorded byte's centre,
+ *           which the writers' truncating quantiser maps back to b;
+ *   out   = decoded where alpha = 1, k where alpha = 0 (both bitwise), else k + alpha * (decoded - k), no FMA.
+ * cell is a power of two <= 32 that divides H and w, 0 <= feather <= 64; out and alpha alias nothing. One launch; the
+ * output is bitwise the same from call to call. */
+int pn_composite_frames(const float* decoded, const float* recorded, const float* cells, float* out, float* alpha,
+                        int64_t frames, int64_t height, int64_t view_width, int64_t cell, int64_t feather, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -101,6 +101,8 @@ SIGNATURES: dict[str, tuple] = {
     "pn_softmax_rows_operand": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _f32, C.c_int, _vp]),
     "pn_render_layout": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "pn_layout_change_mask": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _vp]),
+    "pn_mask_cells": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64, _i64, _vp]),
+    "pn_composite_frames": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _vp]),
 }
 
 

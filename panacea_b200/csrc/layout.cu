@@ -190,6 +190,23 @@ __global__ void __launch_bounds__(MASK_THREADS) dilate_cells_kernel(float* __res
   }
 }
 
+// A user-drawn pixel mask pooled to cells: the pass-1 layout of change_cells_kernel over one uint8 plane per frame.
+__global__ void __launch_bounds__(MASK_THREADS) pixel_cells_kernel(const uint8_t* __restrict__ pixels,
+                                                                   float* __restrict__ out, int H, int Wt, int cell) {
+  const int x = blockIdx.x * MASK_THREADS + threadIdx.x, cy = blockIdx.y, frame = blockIdx.z;
+  bool set = false;
+  if (x < Wt) {
+    const uint8_t* p = pixels + ((size_t)frame * H + (size_t)cy * cell) * Wt + x;
+    for (int r = 0; r < cell; ++r) set |= p[(size_t)r * Wt] != 0;
+  }
+  const unsigned votes = __ballot_sync(0xffffffffu, set);
+  const int lane = threadIdx.x & 31;
+  if (x < Wt && lane % cell == 0) {
+    const unsigned group = cell == 32 ? 0xffffffffu : ((1u << cell) - 1u) << lane;
+    out[((size_t)frame * (H / cell) + cy) * (Wt / cell) + x / cell] = (votes & group) ? 1.f : 0.f;
+  }
+}
+
 }  // namespace pn
 
 extern "C" int pn_layout_change_mask(const float* a, const float* b, float* out, int64_t frames, int64_t height,
@@ -210,6 +227,33 @@ extern "C" int pn_layout_change_mask(const float* a, const float* b, float* out,
   const int64_t Wt = view_width * pn::LAYOUT_VIEWS;
   const dim3 grid((unsigned)((Wt + pn::MASK_THREADS - 1) / pn::MASK_THREADS), (unsigned)(height / cell), (unsigned)frames);
   pn::change_cells_kernel<<<grid, pn::MASK_THREADS, 0, st>>>(a, b, out, (int)height, (int)Wt, (int)cell);
+  PN_CHECK_CUDA(cudaGetLastError());
+  if (dilate > 0) {
+    const int d = (int)(dilate < 65536 ? dilate : 65536);     // a panel has fewer cells per side
+    pn::dilate_cells_kernel<<<(unsigned)(frames * pn::LAYOUT_VIEWS), pn::MASK_THREADS, 0, st>>>(
+        out, (int)(height / cell), (int)(view_width / cell), d);
+    PN_CHECK_CUDA(cudaGetLastError());
+  }
+  return pn::PN_OK;
+}
+
+extern "C" int pn_mask_cells(const uint8_t* pixels, float* out, int64_t frames, int64_t height, int64_t view_width,
+                             int64_t cell, int64_t dilate, void* stream_v) {
+  PN_REQUIRE(pixels && out, "pn_mask_cells: null pointer");
+  PN_REQUIRE(cell >= 1 && cell <= 32 && (cell & (cell - 1)) == 0, "pn_mask_cells: cell %lld is not a power of two <= 32",
+             (long long)cell);
+  PN_REQUIRE(frames > 0 && frames <= 65535 / pn::LAYOUT_VIEWS && height > 0 && view_width > 0 &&
+             height * view_width * pn::LAYOUT_VIEWS <= (int64_t)1 << 31,
+             "pn_mask_cells: bad clip size %lld x %lld x %lld", (long long)frames, (long long)height, (long long)view_width);
+  PN_REQUIRE(height % cell == 0 && view_width % cell == 0, "pn_mask_cells: %lld x %lld is not a multiple of cell %lld",
+             (long long)height, (long long)view_width, (long long)cell);
+  PN_REQUIRE((height / cell) * (view_width / cell) <= pn::MASK_MAX_CELLS, "pn_mask_cells: more than %d cells per panel",
+             pn::MASK_MAX_CELLS);
+  PN_REQUIRE(dilate >= 0, "pn_mask_cells: dilate %lld < 0", (long long)dilate);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+  const int64_t Wt = view_width * pn::LAYOUT_VIEWS;
+  const dim3 grid((unsigned)((Wt + pn::MASK_THREADS - 1) / pn::MASK_THREADS), (unsigned)(height / cell), (unsigned)frames);
+  pn::pixel_cells_kernel<<<grid, pn::MASK_THREADS, 0, st>>>(pixels, out, (int)height, (int)Wt, (int)cell);
   PN_CHECK_CUDA(cudaGetLastError());
   if (dilate > 0) {
     const int d = (int)(dilate < 65536 ? dilate : 65536);     // a panel has fewer cells per side

@@ -13,7 +13,8 @@ embedder is a deterministic stand-in. With the real modules importable, `--datas
 swap them in. `--clips K` generates scenes of K clips chained through their boundary frame, and `--overlap M` chains
 them through M shared frames whose latents each clip keeps from the one before (DESIGN.md section 11).
 `--strength S` edits each item's recorded frames instead of sampling from noise, and with `--layout EDITED.npz
---mask_from ORIGINAL.npz` regenerates only where the edited layout differs from the original (DESIGN.md section 13).
+--mask_from ORIGINAL.npz` regenerates only where the edited layout differs from the original (DESIGN.md section 13);
+`--mask_image` takes a user-drawn mask, and `--composite F` pastes the recorded pixels back outside the edit.
 Overrides use the dotlist form, and a numeric component indexes a list:
 
   torchrun --nproc-per-node 8 -m panacea_b200.inference --base configs.yaml --name run1 --inferdir out --gather
@@ -247,6 +248,12 @@ def get_parser():
     p.add_argument("--mask_from", type=str, default=None,
                    help="original scene file: with --layout EDITED.npz --strength, regenerate only where the layouts differ")
     p.add_argument("--mask_dilate", type=int, default=1, help="latent cells the --mask_from change mask grows by within a panel")
+    p.add_argument("--mask_image", type=str, default=None,
+                   help="user-drawn edit mask: an [H, 6w] image (>= 128 regenerates) for every frame, or a .npy bool/uint8 "
+                        "[T, H, 6w]; needs --strength, grows by --mask_dilate cells and is united with --mask_from")
+    p.add_argument("--composite", type=int, default=None,
+                   help="paste the recorded pixels back outside the edit mask with a feather of F pixels (0 .. 64); needs "
+                        "--strength and --mask_from or --mask_image (DESIGN.md section 13)")
     return p
 
 
@@ -266,6 +273,30 @@ def check_edit_args(opt):
             raise ValueError("--mask_from regenerates part of a recorded clip: it needs --strength")
     if opt.mask_dilate < 0:
         raise ValueError(f"--mask_dilate must be >= 0, got {opt.mask_dilate}")
+
+
+def check_mask_args(opt):
+    """The user-drawn mask and compositing options that cannot be combined; raises ValueError naming the flag."""
+    if opt.mask_image is not None and opt.strength is None:
+        raise ValueError("--mask_image regenerates part of a recorded clip: it needs --strength")
+    if opt.composite is not None:
+        if opt.strength is None:
+            raise ValueError("--composite pastes the recorded pixels back into an edit: it needs --strength")
+        if opt.mask_from is None and opt.mask_image is None:
+            raise ValueError("--composite needs an edit mask (--mask_from or --mask_image): without one every cell is "
+                             "regenerated and nothing is pasted back")
+        if not 0 <= opt.composite <= 64:
+            raise ValueError(f"--composite must lie in 0 .. 64 pixels, got {opt.composite}")
+
+
+def read_mask_image(opt, num_frames: int):
+    """The --mask_image pixels, uint8 [T, H, 6w] on the host, or None; a file that does not fit raises ValueError."""
+    if opt.mask_image is None:
+        return None
+    try:
+        return L.read_edit_mask(opt.mask_image, num_frames, tuple(opt.image_hw))
+    except (ValueError, OSError) as e:
+        raise ValueError(f"--mask_image: {e}") from e
 
 
 def check_scene_args(opt, num_frames: int):
@@ -310,10 +341,12 @@ def main(argv=None):
     if not opt.name:
         raise ValueError("You must specify the experiment name!!")
     check_edit_args(opt)
+    check_mask_args(opt)
     assert opt.bs == 1, "the reference runs batch size 1 (one sequence per rank and step)"
     inferdir = os.path.join(opt.inferdir, opt.name)
     config = load_config(opt.base, unknown)
     check_scene_args(opt, num_frames(config))
+    drawn = read_mask_image(opt, num_frames(config))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world > 1:
         local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -332,6 +365,9 @@ def main(argv=None):
     if opt.mask_from:
         mask = L.change_mask(L.load_scene(opt.mask_from), dataset.scene, dataset.frames(0), tuple(opt.image_hw),
                              opt.mask_dilate, device)
+    if drawn is not None:
+        cells = L.mask_cells(drawn, opt.mask_dilate, device)
+        mask = cells if mask is None else torch.maximum(mask, cells)
     sampler = DistributedSampler(dataset, num_replicas=world, rank=rank, shuffle=False)
     loader = DataLoader(dataset, batch_size=opt.bs, sampler=sampler)
 
@@ -357,7 +393,8 @@ def main(argv=None):
             if key not in ("txt", "filenames"):
                 batch[key] = batch[key].to(device)
         with torch.no_grad():
-            outs = model.log_images(batch) if opt.strength is None else model.edit_images(batch, opt.strength, mask)
+            outs = model.log_images(batch) if opt.strength is None else \
+                model.edit_images(batch, opt.strength, mask, composite=opt.composite)
         filenames = batch["filenames"]
         samples = outs["samples"]
         if opt.gather and world > 1:                           # BASELINE.json configs[2]: NCCL gather of decoded frames

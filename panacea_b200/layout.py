@@ -36,6 +36,7 @@ Scene file keys (arrays; `np.savez`):
                              images: the clip that editing starts from (DESIGN.md section 13)
 
 `change_mask` compares two scenes' renders at latent resolution: where an edited scene differs from its original.
+`read_edit_mask` and `mask_cells` take a mask the user drew instead, and bring it to the same form.
 """
 from __future__ import annotations
 
@@ -416,4 +417,49 @@ def change_mask(scene_a: Scene, scene_b: Scene, frames, image_hw, dilate: int = 
     stream = C.c_void_p(torch.cuda.current_stream(a.device).cuda_stream) if a.is_cuda else None
     _lib.check(_lib.load().pn_layout_change_mask(ptr(a), ptr(b), ptr(out), len(frames), H, w, LATENT_CELL, int(dilate), stream),
                "pn_layout_change_mask")
+    return out
+
+
+def read_edit_mask(path, num_frames: int, image_hw) -> np.ndarray:
+    """A user-drawn edit mask as uint8 [T, H, 6w] on the host, 1 where the clip is to be regenerated. An image file
+    (read as greyscale, a pixel is set when >= 128) is one mask for every frame; a `.npy` file holds one mask per frame,
+    bool or uint8 [T, H, 6w] (nonzero is set), since what is edited moves from frame to frame. Raises ValueError with
+    the expected and the actual value when the shape, dtype or frame count is wrong."""
+    from PIL import Image
+    path = Path(path)
+    H, w = image_hw
+    want = (num_frames, H, len(CAMERA_VIEWS) * w)
+    if path.suffix == ".npy":
+        a = np.load(path, allow_pickle=False)
+        if a.dtype not in (np.bool_, np.uint8):
+            raise ValueError(f"{path.name}: expected a bool or uint8 array, got {a.dtype}")
+        if a.ndim != 3:
+            raise ValueError(f"{path.name}: expected shape {want} (frames, H, 6w), got {a.shape}")
+        if a.shape[0] != num_frames:
+            raise ValueError(f"{path.name}: expected {num_frames} frames, got {a.shape[0]}")
+        if a.shape != want:
+            raise ValueError(f"{path.name}: expected shape {want} (frames, H, 6w), got {a.shape}")
+        return (a != 0).astype(np.uint8)
+    img = np.asarray(Image.open(path).convert("L"))
+    if img.shape != want[1:]:
+        raise ValueError(f"{path.name}: expected a {want[2]} x {want[1]} image, got {img.shape[1]} x {img.shape[0]}")
+    return np.ascontiguousarray(np.broadcast_to((img >= 128).astype(np.uint8), want))
+
+
+def mask_cells(pixels, dilate: int = 1, device="cuda") -> torch.Tensor:
+    """[T, H/8, 6w/8] fp32 in {0, 1} on `device`, the form of `change_mask`: 1 at the latent cells holding a nonzero
+    pixel of `pixels` (uint8 [T, H, 6w], e.g. from `read_edit_mask`), dilated by `dilate` cells within each panel
+    (pn_mask_cells)."""
+    pixels = torch.as_tensor(np.ascontiguousarray(pixels, dtype=np.uint8))
+    _need(pixels.dim() == 3 and pixels.shape[2] % len(CAMERA_VIEWS) == 0, f"expected uint8 [T, H, 6w], got {tuple(pixels.shape)}")
+    T, H, Wt = pixels.shape
+    w = Wt // len(CAMERA_VIEWS)
+    _need(H % LATENT_CELL == 0 and w % LATENT_CELL == 0, f"image size {H} x {w} is not a multiple of {LATENT_CELL}")
+    _need(int(dilate) >= 0, f"dilate must be >= 0, got {dilate}")
+    dev = torch.device(device)
+    src = pixels.to(dev)
+    out = torch.empty(T, H // LATENT_CELL, Wt // LATENT_CELL, dtype=torch.float32, device=dev)
+    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream) if dev.type == "cuda" else None
+    _lib.check(_lib.load().pn_mask_cells(C.c_void_p(src.data_ptr()), C.c_void_p(out.data_ptr()), T, H, w, LATENT_CELL,
+                                         int(dilate), stream), "pn_mask_cells")
     return out

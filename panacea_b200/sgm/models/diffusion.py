@@ -8,6 +8,7 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
+from ...composite import composite_frames
 from ..modules.diffusionmodules.sampling import BoundDenoiser
 from ..modules.diffusionmodules.wrappers import OpenAIWrapperControlLDM3D
 from ..modules.encoders.modules import FrozenOpenCLIPEmbedder, VAEEmbedder
@@ -136,15 +137,22 @@ class DiffusionEngine3D(nn.Module):
         return log, c, uc, N, latent_shape, z
 
     @torch.no_grad()
-    def edit_images(self, batch, strength, mask=None, N=8):
+    def edit_images(self, batch, strength, mask=None, N=8, composite=None):
         """log_images for a recorded clip (DESIGN.md section 13): the sampler starts from the clip's own latent z0 =
         encode(batch["jpg"]) noised to the first sigma of the strength's schedule, z0 + sigma_start eps (eps drawn as
         `sample` draws it), handed over as (z0 + sigma_start eps) / sqrt(1 + sigma_start^2) since the sampler's first
         launch scales by sqrt(1 + sigma_0^2) (upstream's do_img2img). `mask` [N T, h, w] in [0, 1] (None: no blending)
         regenerates only where it is > 0: elsewhere every step's result is the known latent z0 noised to its level, and
-        the final latent is z0 where mask = 0. Returns the log_images keys plus "edit_mask"."""
+        the final latent is z0 where mask = 0. Returns the log_images keys plus "edit_mask".
+
+        `composite` = F pastes the recorded pixels back outside the regenerated cells with a feather of F pixels
+        (panacea_b200/composite.py): "samples" becomes the composite, "decoded_samples" the plain decode and
+        "composite_alpha" [N T, H, 6w] the weight of the decode. It draws nothing from any generator, and needs a mask."""
         if self.input_key not in batch:
             raise KeyError(f"edit_images needs the recorded frames in batch[{self.input_key!r}]")
+        if composite is not None and mask is None:
+            raise ValueError("composite pastes the recorded pixels back outside a mask: an edit without one regenerates "
+                             "every cell, so there is nothing to paste")
         sigma = float(self.sampler.sigmas(strength=strength)[0])                  # rejects a bad strength first
         log, c, uc, N, latent_shape, z = self._log_inputs(batch, N)
         eps = self._initial_noise(c, N * self.num_frames, latent_shape)
@@ -156,6 +164,9 @@ class DiffusionEngine3D(nn.Module):
         log["samples"] = self.decode_first_stage(samples)
         log["sample_latents"] = samples
         log["edit_mask"] = torch.ones(z.shape[0], *z.shape[2:], device=z.device) if mask is None else mask
+        if composite is not None:
+            log["decoded_samples"] = log["samples"]
+            log["samples"], log["composite_alpha"] = composite_frames(log["decoded_samples"], log["inputs"], mask, composite)
         return log
 
     def _image_condition_key(self) -> str:

@@ -8,6 +8,8 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
+import torch
+
 _PKG = Path(__file__).resolve().parent
 LIB_PATH = _PKG / "libpanacea_b200.so"
 
@@ -132,3 +134,16 @@ def check(status: int, what: str) -> None:
     if status != 0:
         msg = load().pn_last_error()
         raise PanaceaNativeError(f"{what} failed with status {status}: {msg.decode() if msg else '?'}")
+
+
+def ptr(t):
+    """A tensor's device address for a `void*` argument (None stays NULL)."""
+    return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def stream(device=None):
+    """torch's current stream on `device` (default: the current device) as a `void*`; None (the default stream) for a
+    device that is not CUDA."""
+    if device is not None and torch.device(device).type != "cuda":
+        return None
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)

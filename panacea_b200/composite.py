@@ -9,11 +9,10 @@ lower for 63 of the 256 bytes). The result does not depend on the precision mode
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 
 from . import _lib
+from ._lib import ptr
 
 MAX_FEATHER = 64
 VIEWS = 6
@@ -39,8 +38,6 @@ def composite_frames(decoded: torch.Tensor, recorded: torch.Tensor, cells: torch
     cel = cells.to(dev, torch.float32).contiguous()
     out = torch.empty_like(dec)
     alpha = torch.empty(F, H, Wt, dtype=torch.float32, device=dev)
-    ptr = lambda t: C.c_void_p(t.data_ptr())
-    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream) if dev.type == "cuda" else None
     _lib.check(_lib.load().pn_composite_frames(ptr(dec), ptr(rec), ptr(cel), ptr(out), ptr(alpha), F, H, Wt // VIEWS,
-                                               H // cells.shape[1], int(feather), stream), "pn_composite_frames")
+                                               H // cells.shape[1], int(feather), _lib.stream(dev)), "pn_composite_frames")
     return out, alpha

@@ -150,23 +150,45 @@ __global__ void __launch_bounds__(LAYOUT_THREADS) render_layout_kernel(
 // ---------------------------------------------------------------- change mask (DESIGN.md section 13)
 constexpr int MASK_THREADS = 256, MASK_MAX_CELLS = 49152;
 
-// Pass 1: one thread per pixel column of a cell row compares the 19 channels of its `cell` pixels; the `cell` lanes of a
-// cell (cell divides 32, so a cell never straddles two warps) combine their verdicts with one ballot.
-__global__ void __launch_bounds__(MASK_THREADS) change_cells_kernel(const float* __restrict__ a,
-                                                                    const float* __restrict__ b, float* __restrict__ out,
-                                                                    int H, int Wt, int cell) {
-  const int x = blockIdx.x * MASK_THREADS + threadIdx.x, cy = blockIdx.y, frame = blockIdx.z;
-  bool differs = false;
-  if (x < Wt) {
+// The per-pixel sources of pass 1. Each tells whether any of the `cell` pixels of column x, rows cy*cell .. cy*cell +
+// cell - 1 of a frame is set. They load through __ldg: a struct member cannot carry the __restrict__ that would let the
+// compiler use the read-only path on its own.
+struct ChangedLayout {          // two 19-channel fp32 renders [T, 19, H, Wt]: set where any channel differs
+  const float* a;
+  const float* b;
+  bool given() const { return a && b; }
+  __device__ __forceinline__ bool operator()(int frame, int cy, int x, int H, int Wt, int cell) const {
     const size_t plane = (size_t)H * Wt;
     const size_t base = (size_t)frame * LAYOUT_CHANNELS * plane + (size_t)cy * cell * Wt + x;
+    bool differs = false;
     for (int c = 0; c < LAYOUT_CHANNELS; ++c)
       for (int r = 0; r < cell; ++r) {
         const size_t i = base + c * plane + (size_t)r * Wt;
-        differs |= a[i] != b[i];
+        differs |= __ldg(a + i) != __ldg(b + i);
       }
+    return differs;
   }
-  const unsigned votes = __ballot_sync(0xffffffffu, differs);
+};
+
+struct DrawnPixels {            // a user-drawn uint8 mask [T, H, Wt]: set where nonzero
+  const uint8_t* pixels;
+  bool given() const { return pixels; }
+  __device__ __forceinline__ bool operator()(int frame, int cy, int x, int H, int Wt, int cell) const {
+    const uint8_t* p = pixels + ((size_t)frame * H + (size_t)cy * cell) * Wt + x;
+    bool set = false;
+    for (int r = 0; r < cell; ++r) set |= __ldg(p + (size_t)r * Wt) != 0;
+    return set;
+  }
+};
+
+// Pass 1: one thread per pixel column of a cell row asks the source about its `cell` pixels; the `cell` lanes of a cell
+// (cell divides 32, so a cell never straddles two warps) combine their verdicts with one ballot.
+template <class Source>
+__global__ void __launch_bounds__(MASK_THREADS) pool_cells_kernel(const Source src, float* __restrict__ out, int H, int Wt,
+                                                                  int cell) {
+  const int x = blockIdx.x * MASK_THREADS + threadIdx.x, cy = blockIdx.y, frame = blockIdx.z;
+  const bool set = x < Wt && src(frame, cy, x, H, Wt, cell);
+  const unsigned votes = __ballot_sync(0xffffffffu, set);
   const int lane = threadIdx.x & 31;
   if (x < Wt && lane % cell == 0) {
     const unsigned group = cell == 32 ? 0xffffffffu : ((1u << cell) - 1u) << lane;
@@ -190,78 +212,45 @@ __global__ void __launch_bounds__(MASK_THREADS) dilate_cells_kernel(float* __res
   }
 }
 
-// A user-drawn pixel mask pooled to cells: the pass-1 layout of change_cells_kernel over one uint8 plane per frame.
-__global__ void __launch_bounds__(MASK_THREADS) pixel_cells_kernel(const uint8_t* __restrict__ pixels,
-                                                                   float* __restrict__ out, int H, int Wt, int cell) {
-  const int x = blockIdx.x * MASK_THREADS + threadIdx.x, cy = blockIdx.y, frame = blockIdx.z;
-  bool set = false;
-  if (x < Wt) {
-    const uint8_t* p = pixels + ((size_t)frame * H + (size_t)cy * cell) * Wt + x;
-    for (int r = 0; r < cell; ++r) set |= p[(size_t)r * Wt] != 0;
+// The checks, pass 1 over `src` and pass 2 of both cell-mask entry points; `fn` names the entry point in every message.
+template <class Source>
+static int cell_mask(const char* fn, const Source src, float* out, int64_t frames, int64_t height, int64_t view_width,
+                     int64_t cell, int64_t dilate, void* stream_v) {
+  PN_REQUIRE(src.given() && out, "%s: null pointer", fn);
+  PN_REQUIRE(cell >= 1 && cell <= 32 && (cell & (cell - 1)) == 0, "%s: cell %lld is not a power of two <= 32", fn,
+             (long long)cell);
+  PN_REQUIRE(frames > 0 && frames <= 65535 / LAYOUT_VIEWS && height > 0 && view_width > 0 &&
+             height * view_width * LAYOUT_VIEWS <= (int64_t)1 << 31,
+             "%s: bad clip size %lld x %lld x %lld", fn, (long long)frames, (long long)height, (long long)view_width);
+  PN_REQUIRE(height % cell == 0 && view_width % cell == 0, "%s: %lld x %lld is not a multiple of cell %lld", fn,
+             (long long)height, (long long)view_width, (long long)cell);
+  PN_REQUIRE((height / cell) * (view_width / cell) <= MASK_MAX_CELLS, "%s: more than %d cells per panel", fn, MASK_MAX_CELLS);
+  PN_REQUIRE(dilate >= 0, "%s: dilate %lld < 0", fn, (long long)dilate);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+  const int64_t Wt = view_width * LAYOUT_VIEWS;
+  const dim3 grid((unsigned)((Wt + MASK_THREADS - 1) / MASK_THREADS), (unsigned)(height / cell), (unsigned)frames);
+  pool_cells_kernel<<<grid, MASK_THREADS, 0, st>>>(src, out, (int)height, (int)Wt, (int)cell);
+  PN_CHECK_CUDA(cudaGetLastError());
+  if (dilate > 0) {
+    const int d = (int)(dilate < 65536 ? dilate : 65536);     // a panel has fewer cells per side
+    dilate_cells_kernel<<<(unsigned)(frames * LAYOUT_VIEWS), MASK_THREADS, 0, st>>>(out, (int)(height / cell),
+                                                                                     (int)(view_width / cell), d);
+    PN_CHECK_CUDA(cudaGetLastError());
   }
-  const unsigned votes = __ballot_sync(0xffffffffu, set);
-  const int lane = threadIdx.x & 31;
-  if (x < Wt && lane % cell == 0) {
-    const unsigned group = cell == 32 ? 0xffffffffu : ((1u << cell) - 1u) << lane;
-    out[((size_t)frame * (H / cell) + cy) * (Wt / cell) + x / cell] = (votes & group) ? 1.f : 0.f;
-  }
+  return PN_OK;
 }
 
 }  // namespace pn
 
 extern "C" int pn_layout_change_mask(const float* a, const float* b, float* out, int64_t frames, int64_t height,
                                      int64_t view_width, int64_t cell, int64_t dilate, void* stream_v) {
-  PN_REQUIRE(a && b && out, "pn_layout_change_mask: null pointer");
-  PN_REQUIRE(cell >= 1 && cell <= 32 && (cell & (cell - 1)) == 0, "pn_layout_change_mask: cell %lld is not a power of two <= 32",
-             (long long)cell);
-  PN_REQUIRE(frames > 0 && frames <= 65535 / pn::LAYOUT_VIEWS && height > 0 && view_width > 0 &&
-             height * view_width * pn::LAYOUT_VIEWS <= (int64_t)1 << 31,
-             "pn_layout_change_mask: bad clip size %lld x %lld x %lld", (long long)frames, (long long)height,
-             (long long)view_width);
-  PN_REQUIRE(height % cell == 0 && view_width % cell == 0, "pn_layout_change_mask: %lld x %lld is not a multiple of cell %lld",
-             (long long)height, (long long)view_width, (long long)cell);
-  PN_REQUIRE((height / cell) * (view_width / cell) <= pn::MASK_MAX_CELLS, "pn_layout_change_mask: more than %d cells per panel",
-             pn::MASK_MAX_CELLS);
-  PN_REQUIRE(dilate >= 0, "pn_layout_change_mask: dilate %lld < 0", (long long)dilate);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  const int64_t Wt = view_width * pn::LAYOUT_VIEWS;
-  const dim3 grid((unsigned)((Wt + pn::MASK_THREADS - 1) / pn::MASK_THREADS), (unsigned)(height / cell), (unsigned)frames);
-  pn::change_cells_kernel<<<grid, pn::MASK_THREADS, 0, st>>>(a, b, out, (int)height, (int)Wt, (int)cell);
-  PN_CHECK_CUDA(cudaGetLastError());
-  if (dilate > 0) {
-    const int d = (int)(dilate < 65536 ? dilate : 65536);     // a panel has fewer cells per side
-    pn::dilate_cells_kernel<<<(unsigned)(frames * pn::LAYOUT_VIEWS), pn::MASK_THREADS, 0, st>>>(
-        out, (int)(height / cell), (int)(view_width / cell), d);
-    PN_CHECK_CUDA(cudaGetLastError());
-  }
-  return pn::PN_OK;
+  return pn::cell_mask("pn_layout_change_mask", pn::ChangedLayout{a, b}, out, frames, height, view_width, cell, dilate,
+                       stream_v);
 }
 
 extern "C" int pn_mask_cells(const uint8_t* pixels, float* out, int64_t frames, int64_t height, int64_t view_width,
                              int64_t cell, int64_t dilate, void* stream_v) {
-  PN_REQUIRE(pixels && out, "pn_mask_cells: null pointer");
-  PN_REQUIRE(cell >= 1 && cell <= 32 && (cell & (cell - 1)) == 0, "pn_mask_cells: cell %lld is not a power of two <= 32",
-             (long long)cell);
-  PN_REQUIRE(frames > 0 && frames <= 65535 / pn::LAYOUT_VIEWS && height > 0 && view_width > 0 &&
-             height * view_width * pn::LAYOUT_VIEWS <= (int64_t)1 << 31,
-             "pn_mask_cells: bad clip size %lld x %lld x %lld", (long long)frames, (long long)height, (long long)view_width);
-  PN_REQUIRE(height % cell == 0 && view_width % cell == 0, "pn_mask_cells: %lld x %lld is not a multiple of cell %lld",
-             (long long)height, (long long)view_width, (long long)cell);
-  PN_REQUIRE((height / cell) * (view_width / cell) <= pn::MASK_MAX_CELLS, "pn_mask_cells: more than %d cells per panel",
-             pn::MASK_MAX_CELLS);
-  PN_REQUIRE(dilate >= 0, "pn_mask_cells: dilate %lld < 0", (long long)dilate);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
-  const int64_t Wt = view_width * pn::LAYOUT_VIEWS;
-  const dim3 grid((unsigned)((Wt + pn::MASK_THREADS - 1) / pn::MASK_THREADS), (unsigned)(height / cell), (unsigned)frames);
-  pn::pixel_cells_kernel<<<grid, pn::MASK_THREADS, 0, st>>>(pixels, out, (int)height, (int)Wt, (int)cell);
-  PN_CHECK_CUDA(cudaGetLastError());
-  if (dilate > 0) {
-    const int d = (int)(dilate < 65536 ? dilate : 65536);     // a panel has fewer cells per side
-    pn::dilate_cells_kernel<<<(unsigned)(frames * pn::LAYOUT_VIEWS), pn::MASK_THREADS, 0, st>>>(
-        out, (int)(height / cell), (int)(view_width / cell), d);
-    PN_CHECK_CUDA(cudaGetLastError());
-  }
-  return pn::PN_OK;
+  return pn::cell_mask("pn_mask_cells", pn::DrawnPixels{pixels}, out, frames, height, view_width, cell, dilate, stream_v);
 }
 
 extern "C" int pn_render_layout(const float* prims, const int32_t* panel_offsets, const double* rays, float* out,

@@ -40,3 +40,12 @@ def gather_on_rank0(x: torch.Tensor):
     outs = [torch.empty_like(x) for _ in range(dist.get_world_size())] if dist.get_rank() == 0 else None
     dist.gather(x, outs, dst=0)
     return outs
+
+
+def gather_named_on_rank0(x: torch.Tensor, names):
+    """`gather_on_rank0` of `x`, with each rank's `names` (any picklable value, e.g. its frame file names) gathered
+    alongside. Returns [(x of rank r, names of rank r) for every rank r] on rank 0 and [] elsewhere."""
+    gathered = gather_on_rank0(x.contiguous())
+    all_names = [None] * dist.get_world_size()
+    dist.all_gather_object(all_names, names)
+    return [] if gathered is None else list(zip(gathered, all_names))

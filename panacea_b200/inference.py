@@ -40,8 +40,16 @@ from torch.utils.data.distributed import DistributedSampler
 from . import dist_utils as D
 from . import frame_io as IO
 from . import layout as L
+from .composite import MAX_FEATHER
 from .scene import check_overlap, cond_index, condition_from_frame, scene_frame_number, scene_length
 from .sgm.util import instantiate_from_config
+
+
+def _check_scene(clips, overlap, num_frames):
+    """A dataset item of `clips` clips of `num_frames` frames sharing `overlap` (scene.check_overlap)."""
+    if clips < 1:
+        raise ValueError(f"clips must be >= 1, got {clips}")
+    check_overlap(overlap, num_frames)
 
 
 class SyntheticBEVDataset(Dataset):
@@ -58,9 +66,7 @@ class SyntheticBEVDataset(Dataset):
     def __init__(self, num_sequences=2, num_frames=8, image_hw=(256, 512), use_last_frame=True, seed=0, clips=1,
                  overlap=None):
         self.n, self.T, (self.h, self.w), self.use_last_frame, self.seed = num_sequences, num_frames, image_hw, use_last_frame, seed
-        if clips < 1:
-            raise ValueError(f"clips must be >= 1, got {clips}")
-        check_overlap(overlap, num_frames)
+        _check_scene(clips, overlap, num_frames)
         self.clips, self.overlap = clips, overlap
 
     def __len__(self):
@@ -104,9 +110,7 @@ class LayoutDataset(Dataset):
 
     def __init__(self, path, num_frames=8, image_hw=(256, 512), use_last_frame=True, clips=1, cond_frame=None,
                  device="cuda", edit=False, overlap=None):
-        if clips < 1:
-            raise ValueError(f"clips must be >= 1, got {clips}")
-        check_overlap(overlap, num_frames)
+        _check_scene(clips, overlap, num_frames)
         self.path, self.T, (self.h, self.w) = Path(path), num_frames, tuple(image_hw)
         self.use_last_frame, self.clips, self.device, self.edit, self.overlap = use_last_frame, clips, device, edit, overlap
         self.scene = L.load_scene(path)
@@ -252,13 +256,14 @@ def get_parser():
                    help="user-drawn edit mask: an [H, 6w] image (>= 128 regenerates) for every frame, or a .npy bool/uint8 "
                         "[T, H, 6w]; needs --strength, grows by --mask_dilate cells and is united with --mask_from")
     p.add_argument("--composite", type=int, default=None,
-                   help="paste the recorded pixels back outside the edit mask with a feather of F pixels (0 .. 64); needs "
-                        "--strength and --mask_from or --mask_image (DESIGN.md section 13)")
+                   help=f"paste the recorded pixels back outside the edit mask with a feather of F pixels (0 .. {MAX_FEATHER}); "
+                        "needs --strength and --mask_from or --mask_image (DESIGN.md section 13)")
     return p
 
 
-def check_edit_args(opt):
-    """The editing options that cannot be combined; raises ValueError with the reason."""
+def check_args(opt):
+    """The editing, mask and compositing options that cannot be combined, whatever the clip length; raises ValueError
+    naming the flag. main runs this before it reads the config."""
     if opt.strength is not None:
         if not 0.0 < opt.strength <= 1.0:
             raise ValueError(f"--strength must lie in (0, 1], got {opt.strength}")
@@ -273,10 +278,6 @@ def check_edit_args(opt):
             raise ValueError("--mask_from regenerates part of a recorded clip: it needs --strength")
     if opt.mask_dilate < 0:
         raise ValueError(f"--mask_dilate must be >= 0, got {opt.mask_dilate}")
-
-
-def check_mask_args(opt):
-    """The user-drawn mask and compositing options that cannot be combined; raises ValueError naming the flag."""
     if opt.mask_image is not None and opt.strength is None:
         raise ValueError("--mask_image regenerates part of a recorded clip: it needs --strength")
     if opt.composite is not None:
@@ -285,26 +286,23 @@ def check_mask_args(opt):
         if opt.mask_from is None and opt.mask_image is None:
             raise ValueError("--composite needs an edit mask (--mask_from or --mask_image): without one every cell is "
                              "regenerated and nothing is pasted back")
-        if not 0 <= opt.composite <= 64:
-            raise ValueError(f"--composite must lie in 0 .. 64 pixels, got {opt.composite}")
+        if not 0 <= opt.composite <= MAX_FEATHER:
+            raise ValueError(f"--composite must lie in 0 .. {MAX_FEATHER} pixels, got {opt.composite}")
 
 
-def read_mask_image(opt, num_frames: int):
-    """The --mask_image pixels, uint8 [T, H, 6w] on the host, or None; a file that does not fit raises ValueError."""
+def check_clip_args(opt, num_frames: int):
+    """The scene and mask options checked against clips of `num_frames` frames, before any device work; raises
+    ValueError naming the flag. Returns the --mask_image pixels, uint8 [T, H, 6w] on the host, or None."""
+    if opt.overlap is not None:
+        if opt.clips < 2:
+            raise ValueError(f"--overlap shares frames between consecutive clips: it needs --clips >= 2, got {opt.clips}")
+        check_overlap(opt.overlap, num_frames)
     if opt.mask_image is None:
         return None
     try:
         return L.read_edit_mask(opt.mask_image, num_frames, tuple(opt.image_hw))
     except (ValueError, OSError) as e:
         raise ValueError(f"--mask_image: {e}") from e
-
-
-def check_scene_args(opt, num_frames: int):
-    """The scene options that cannot work with clips of `num_frames` frames; raises ValueError with the reason."""
-    if opt.overlap is not None:
-        if opt.clips < 2:
-            raise ValueError(f"--overlap shares frames between consecutive clips: it needs --clips >= 2, got {opt.clips}")
-        check_overlap(opt.overlap, num_frames)
 
 
 def num_frames(config) -> int:
@@ -340,13 +338,11 @@ def main(argv=None):
     opt, unknown = get_parser().parse_known_args(argv)
     if not opt.name:
         raise ValueError("You must specify the experiment name!!")
-    check_edit_args(opt)
-    check_mask_args(opt)
+    check_args(opt)
     assert opt.bs == 1, "the reference runs batch size 1 (one sequence per rank and step)"
     inferdir = os.path.join(opt.inferdir, opt.name)
     config = load_config(opt.base, unknown)
-    check_scene_args(opt, num_frames(config))
-    drawn = read_mask_image(opt, num_frames(config))
+    drawn = check_clip_args(opt, num_frames(config))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world > 1:
         local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -383,7 +379,7 @@ def main(argv=None):
     for idx, batch in enumerate(loader):
         start = time.time()
         if opt.clips > 1:
-            written += _run_scene(model, batch, opt, inferdir, rank, world, device)
+            written += _run_scene(model, batch, opt, inferdir, world, device)
             all_time += time.time() - start
             if rank == 0:
                 print(f"idx {idx}: time per scene {time.time() - start:.2f}s ({opt.clips} clips), avg {all_time / (idx + 1):.2f}s",
@@ -398,12 +394,8 @@ def main(argv=None):
         filenames = batch["filenames"]
         samples = outs["samples"]
         if opt.gather and world > 1:                           # BASELINE.json configs[2]: NCCL gather of decoded frames
-            gathered = D.gather_on_rank0(samples.contiguous())
-            names = [None] * world
-            dist.all_gather_object(names, filenames)
-            if rank == 0:
-                for r in range(world):
-                    written += IO.logs_frames(gathered[r], os.path.join(inferdir, "fake"), names[r])
+            for frames, names in D.gather_named_on_rank0(samples, filenames):
+                written += IO.logs_frames(frames, os.path.join(inferdir, "fake"), names)
         else:
             written += IO.logs_frames(samples, os.path.join(inferdir, "fake"), filenames)
         written += IO.logs_all_images(outs, os.path.join(inferdir, "allimages"), filenames)
@@ -417,7 +409,7 @@ def main(argv=None):
     return written
 
 
-def _run_scene(model, item, opt, inferdir, rank, world, device) -> list[str]:
+def _run_scene(model, item, opt, inferdir, world, device) -> list[str]:
     """One scene of `opt.clips` clips (`DiffusionEngine3D.sample_scene`, sharing `opt.overlap` frames), written as one
     chronological sequence per camera plus one PNG strip and one GIF; `--gather` gathers one scene per rank on rank 0."""
     clips = item["clips"]
@@ -427,12 +419,7 @@ def _run_scene(model, item, opt, inferdir, rank, world, device) -> list[str]:
         out = model.sample_scene(clips, use_last_frame=opt.use_last_frame, overlap=opt.overlap)
     frames, names = out["samples"], out["filenames"]
     if opt.gather and world > 1:
-        gathered = D.gather_on_rank0(frames.to(device).contiguous())
-        all_names = [None] * world
-        dist.all_gather_object(all_names, names)
-        if rank != 0:
-            return []
-        return [w for r in range(world) for w in IO.logs_scene(gathered[r], inferdir, all_names[r])]
+        return [w for f, n in D.gather_named_on_rank0(frames.to(device), names) for w in IO.logs_scene(f, inferdir, n)]
     return IO.logs_scene(frames, inferdir, names)
 
 

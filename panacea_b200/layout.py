@@ -40,7 +40,6 @@ Scene file keys (arrays; `np.savez`):
 """
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import dataclass
 from pathlib import Path
 
@@ -48,6 +47,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._lib import ptr
 from .frame_io import CAMERA_VIEWS
 
 # nuscenes_datasets_video.py:127-130 (this list, not the one at :81, is the class order of channels 3..12)
@@ -394,11 +394,20 @@ def render_layout(scene: Scene, frames, H: int, w: int, device="cuda") -> torch.
     d_prims = torch.from_numpy(prims).to(dev)
     d_off = torch.from_numpy(offsets).to(dev)
     d_rays = torch.from_numpy(ray_params(scene, H, w)).to(dev)
-    ptr = lambda t: C.c_void_p(t.data_ptr())
-    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream) if dev.type == "cuda" else None
+    _lib.check(_lib.load().pn_render_layout(ptr(d_prims), ptr(d_off), ptr(d_rays), ptr(out), len(frames), H, w,
+                                            _lib.stream(dev)), "pn_render_layout")
+    return out
+
+
+def _cell_mask(entry: str, T: int, H: int, w: int, dilate: int, sources) -> torch.Tensor:
+    """[T, H/8, 6w/8] fp32 in {0, 1} from the cell-mask entry point `entry` over the device tensors `sources()`, which
+    are made only once the size and `dilate` have passed their checks; dilated by `dilate` cells within each panel."""
+    _need(H % LATENT_CELL == 0 and w % LATENT_CELL == 0, f"image size {H} x {w} is not a multiple of {LATENT_CELL}")
+    _need(int(dilate) >= 0, f"dilate must be >= 0, got {dilate}")
+    src = sources()
+    out = torch.empty(T, H // LATENT_CELL, len(CAMERA_VIEWS) * w // LATENT_CELL, dtype=torch.float32, device=src[0].device)
     lib = _lib.load()
-    _lib.check(lib.pn_render_layout(ptr(d_prims), ptr(d_off), ptr(d_rays), ptr(out), len(frames), H, w, stream),
-               "pn_render_layout")
+    _lib.check(getattr(lib, entry)(*map(ptr, src), ptr(out), T, H, w, LATENT_CELL, int(dilate), _lib.stream(out.device)), entry)
     return out
 
 
@@ -408,16 +417,9 @@ def change_mask(scene_a: Scene, scene_b: Scene, frames, image_hw, dilate: int = 
     if scene_a.num_frames != scene_b.num_frames:
         raise SceneError(f"the scenes hold {scene_a.num_frames} and {scene_b.num_frames} frames; a change mask needs the same count")
     H, w = image_hw
-    _need(H % LATENT_CELL == 0 and w % LATENT_CELL == 0, f"image size {H} x {w} is not a multiple of {LATENT_CELL}")
-    _need(int(dilate) >= 0, f"dilate must be >= 0, got {dilate}")
     frames = list(frames)
-    a, b = (render_layout(sc, frames, H, w, device) for sc in (scene_a, scene_b))
-    out = torch.empty(len(frames), H // LATENT_CELL, len(CAMERA_VIEWS) * w // LATENT_CELL, dtype=torch.float32, device=a.device)
-    ptr = lambda t: C.c_void_p(t.data_ptr())
-    stream = C.c_void_p(torch.cuda.current_stream(a.device).cuda_stream) if a.is_cuda else None
-    _lib.check(_lib.load().pn_layout_change_mask(ptr(a), ptr(b), ptr(out), len(frames), H, w, LATENT_CELL, int(dilate), stream),
-               "pn_layout_change_mask")
-    return out
+    return _cell_mask("pn_layout_change_mask", len(frames), H, w, dilate,
+                      lambda: [render_layout(sc, frames, H, w, device) for sc in (scene_a, scene_b)])
 
 
 def read_edit_mask(path, num_frames: int, image_hw) -> np.ndarray:
@@ -453,13 +455,4 @@ def mask_cells(pixels, dilate: int = 1, device="cuda") -> torch.Tensor:
     pixels = torch.as_tensor(np.ascontiguousarray(pixels, dtype=np.uint8))
     _need(pixels.dim() == 3 and pixels.shape[2] % len(CAMERA_VIEWS) == 0, f"expected uint8 [T, H, 6w], got {tuple(pixels.shape)}")
     T, H, Wt = pixels.shape
-    w = Wt // len(CAMERA_VIEWS)
-    _need(H % LATENT_CELL == 0 and w % LATENT_CELL == 0, f"image size {H} x {w} is not a multiple of {LATENT_CELL}")
-    _need(int(dilate) >= 0, f"dilate must be >= 0, got {dilate}")
-    dev = torch.device(device)
-    src = pixels.to(dev)
-    out = torch.empty(T, H // LATENT_CELL, Wt // LATENT_CELL, dtype=torch.float32, device=dev)
-    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream) if dev.type == "cuda" else None
-    _lib.check(_lib.load().pn_mask_cells(C.c_void_p(src.data_ptr()), C.c_void_p(out.data_ptr()), T, H, w, LATENT_CELL,
-                                         int(dilate), stream), "pn_mask_cells")
-    return out
+    return _cell_mask("pn_mask_cells", T, H, Wt // len(CAMERA_VIEWS), dilate, lambda: [pixels.to(device)])

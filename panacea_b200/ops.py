@@ -11,20 +11,13 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._lib import ptr as _ptr, stream as _stream
 
 BF16 = torch.bfloat16
 F32 = torch.float32
 OP_BF16, OP_SPLIT3, OP_F32, OP_SPLIT3_B = 0, 1, 2, 3      # include/panacea_b200.h pn_operand_mode
 # include/panacea_b200.h pn_sampler_mode
 SAMPLER_EULER, SAMPLER_HEUN, SAMPLER_LMS, SAMPLER_DPM, SAMPLER_DPM_2M, SAMPLER_SCALE = range(6)
-
-
-def _ptr(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _req(cond, msg):

@@ -1,8 +1,9 @@
 """`DiffusionEngine3D` — the engine glue of the reference (sgm/models/diffusion.py:30-377) without Lightning: builds
 network + wrapper, denoiser, sampler, conditioner and first stage from the `model.params` block of
 configs/inference_nuscenes.yaml and runs the inference control flow `log_images -> sample -> decode_first_stage`
-(SURVEY.md section 8f, row N1). Training, EMA, optimisers and logging of text images are not part of the inference
-path and are not mirrored. The denoising loop inside `sample` is the hot path of this repository (sm_90a kernels)."""
+(SURVEY.md section 8f, row N1); every clip, generated, edited or outpainted, goes through `_sample_clip`. Training, EMA,
+optimisers and logging of text images are not part of the inference path and are not mirrored. The denoising loop
+inside the sampler call is the hot path of this repository (sm_90a kernels)."""
 from __future__ import annotations
 
 import torch
@@ -74,16 +75,8 @@ class DiffusionEngine3D(nn.Module):
     def encode_first_stage(self, x):
         return self.scale_factor * self.first_stage_model.encode(x)                # diffusion.py:145-150
 
-    @torch.no_grad()
-    def sample(self, cond, uc=None, batch_size=16, shape=None, randn=None, **kwargs):
-        """diffusion.py:233-255. `randn` (optional) replaces the CPU-generator draw for tests."""
-        return self.sampler(BoundDenoiser(self.denoiser, self.model), self._initial_noise(cond, batch_size, shape, randn), cond,
-                            uc=uc)
-
-    def _initial_noise(self, cond, batch_size, shape, randn=None):
-        if randn is None:
-            randn = torch.randn(batch_size, *shape)                                 # CPU generator, like the reference (:242)
-        randn = randn.to(self.device)
+    def _initial_noise(self, cond, batch_size, shape):
+        randn = torch.randn(batch_size, *shape).to(self.device)                    # CPU generator, like the reference (:242)
         if self.share_noise_level > 0.0:
             last = cond["concat"].to(self.device)[-1]
             randn = randn + last.unsqueeze(0).expand(self.num_frames, *last.shape).repeat(randn.shape[0] // self.num_frames, 1, 1, 1) \
@@ -94,11 +87,27 @@ class DiffusionEngine3D(nn.Module):
     def log_images(self, batch, N=8, sample=True, ucg_keys=None, **kwargs):
         """diffusion.py:300-377 for the SD-2.1 branch the config takes (unconditional prompt = ""), without the text/cond
         renderings (log_conditionings draws strings with PIL fonts — not part of the data path)."""
-        log, c, uc, N, latent_shape, _ = self._log_inputs(batch, N)
-        if sample:
-            samples = self.sample(c, shape=latent_shape, uc=uc, batch_size=N * self.num_frames)
-            log["samples"] = self.decode_first_stage(samples)
-            log["sample_latents"] = samples
+        if not sample:
+            return self._log_inputs(batch, N)[0]
+        return self._sample_clip(batch, N)
+
+    def _sample_clip(self, batch, N, strength=1.0, known=None, mask=None, edit_sigma=None):
+        """The path of every clip: _log_inputs, the start latent, one sampler call (diffusion.py:233-255 `sample`),
+        decode. The start latent is the initial noise eps, or with `edit_sigma` = sigma the encoded clip z0 noised to
+        sigma and scaled for the sampler's first launch, (z0 + sigma eps) / sqrt(1 + sigma^2); an edit's `mask` is then
+        reshaped to [N T, h, w] and keeps `known` = z0 where it is 0. Returns the log with "samples" and
+        "sample_latents", and for an edit "edit_mask" (all ones without a mask)."""
+        log, c, uc, N, latent_shape, z = self._log_inputs(batch, N)
+        x = self._initial_noise(c, N * self.num_frames, latent_shape)
+        if edit_sigma is not None:
+            x = (z + edit_sigma * x) / (1.0 + edit_sigma ** 2) ** 0.5
+            if mask is not None:
+                known, mask = z, mask.to(self.device, torch.float32).reshape(z.shape[0], *z.shape[2:])
+        samples = self.sampler(BoundDenoiser(self.denoiser, self.model), x, c, uc=uc, strength=strength, known=known, mask=mask)
+        log["samples"] = self.decode_first_stage(samples)
+        log["sample_latents"] = samples
+        if edit_sigma is not None:
+            log["edit_mask"] = torch.ones(z.shape[0], *z.shape[2:], device=z.device) if mask is None else mask
         return log
 
     def _log_inputs(self, batch, N):
@@ -154,19 +163,11 @@ class DiffusionEngine3D(nn.Module):
             raise ValueError("composite pastes the recorded pixels back outside a mask: an edit without one regenerates "
                              "every cell, so there is nothing to paste")
         sigma = float(self.sampler.sigmas(strength=strength)[0])                  # rejects a bad strength first
-        log, c, uc, N, latent_shape, z = self._log_inputs(batch, N)
-        eps = self._initial_noise(c, N * self.num_frames, latent_shape)
-        x = (z + sigma * eps) / (1.0 + sigma ** 2) ** 0.5
-        if mask is not None:
-            mask = mask.to(self.device, torch.float32).reshape(z.shape[0], *z.shape[2:])
-        samples = self.sampler(BoundDenoiser(self.denoiser, self.model), x, c, uc=uc, strength=strength,
-                               known=None if mask is None else z, mask=mask)
-        log["samples"] = self.decode_first_stage(samples)
-        log["sample_latents"] = samples
-        log["edit_mask"] = torch.ones(z.shape[0], *z.shape[2:], device=z.device) if mask is None else mask
+        log = self._sample_clip(batch, N, strength, mask=mask, edit_sigma=sigma)
         if composite is not None:
             log["decoded_samples"] = log["samples"]
-            log["samples"], log["composite_alpha"] = composite_frames(log["decoded_samples"], log["inputs"], mask, composite)
+            log["samples"], log["composite_alpha"] = composite_frames(log["decoded_samples"], log["inputs"], log["edit_mask"],
+                                                                      composite)
         return log
 
     def _image_condition_key(self) -> str:
@@ -182,12 +183,7 @@ class DiffusionEngine3D(nn.Module):
         sampler blends every step's result toward known + sigma xi there, so the final latent is `known` exactly) and
         generated where it is 1. The known region's Philox seed is drawn from the CPU generator after the churn seed.
         Other `log_images` keywords are accepted and ignored, as `log_images` ignores its own."""
-        log, c, uc, N, latent_shape, _ = self._log_inputs(batch, N)
-        x = self._initial_noise(c, N * self.num_frames, latent_shape)
-        samples = self.sampler(BoundDenoiser(self.denoiser, self.model), x, c, uc=uc, known=known, mask=mask)
-        log["samples"] = self.decode_first_stage(samples)
-        log["sample_latents"] = samples
-        return log
+        return self._sample_clip(batch, N, known=known, mask=mask)
 
     @torch.no_grad()
     def sample_scene(self, batches, use_last_frame=True, overlap=None, **kwargs):

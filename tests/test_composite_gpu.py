@@ -6,7 +6,8 @@
   * pn_mask_cells bitwise against the restatement;
   * both kernels bitwise the same over two calls;
   * on the small model of the scene tests: a composited edit's plain decode is bitwise the uncomposited edit, its
-    frames quantise to the recorded bytes where alpha = 0 and are the decode where alpha = 1;
+    frames quantise to the recorded bytes where alpha = 0 and are the decode where alpha = 1, and under one seed it is
+    bitwise the edit composed by hand from its steps;
   * the command line with a layout change mask and a drawn mask writes a lossless `samples` strip whose pixels are the
     recorded bytes outside the mask and its ramp."""
 import numpy as np
@@ -101,6 +102,31 @@ def test_a_composited_edit_keeps_the_recorded_bytes_outside_the_mask(tmp_path):
     s, d = log["samples"].permute(0, 2, 3, 1).cpu().numpy(), plain["samples"].permute(0, 2, 3, 1).cpu().numpy()
     assert np.array_equal(s[one], d[one])
     assert (np.stack([_to_uint8_hwc(f) for f in plain["samples"]])[zero] != rec[zero]).any()   # the decode alone is not
+
+
+def test_a_composited_edit_is_the_edit_by_hand(tmp_path):
+    """Under one seed, edit_images with a change mask and composite=8 is bitwise _log_inputs -> _initial_noise ->
+    (z0 + sigma eps) / sqrt(1 + sigma^2) -> sampler(strength, known=z0, mask) -> decode -> composite_frames: this pins
+    the edit's draws (the encoder's posterior sample, the initial noise, the churn seed, the known region's seed)."""
+    from panacea_b200.sgm.modules.diffusionmodules.sampling import BoundDenoiser
+    orig, edited = _scene_pair(tmp_path)
+    ds, batch = _layout_batch(edited)
+    mask = L.change_mask(L.load_scene(orig), ds.scene, ds.frames(0), (64, 128), 1)
+    m, _ = _small("bf16")
+    torch.manual_seed(9)
+    log = m.edit_images(batch, 0.6, mask=mask, composite=8)
+    torch.manual_seed(9)
+    ref, c, uc, N, shape, z0 = m._log_inputs(batch, 8)
+    eps = m._initial_noise(c, N * T, shape)
+    sigma = float(m.sampler.sigmas(strength=0.6)[0])
+    x = (z0 + sigma * eps) / (1.0 + sigma ** 2) ** 0.5
+    lat = m.sampler(BoundDenoiser(m.denoiser, m.model), x, c, uc=uc, strength=0.6, known=z0, mask=mask)
+    dec = m.decode_first_stage(lat)
+    frames, alpha = composite_frames(dec, ref["inputs"], mask, 8)
+    assert torch.equal(log["inputs"], ref["inputs"]) and torch.equal(log["edit_mask"], mask)
+    assert torch.equal(log["sample_latents"], lat) and torch.equal(log["decoded_samples"], dec)
+    assert torch.equal(log["samples"], frames) and torch.equal(log["composite_alpha"], alpha)
+    assert not torch.equal(frames, dec)
 
 
 def test_inference_entry_point_composites_a_drawn_and_a_layout_mask(tmp_path):

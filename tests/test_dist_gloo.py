@@ -1,4 +1,5 @@
-"""world_size-2 gloo test of the N>1 path's host logic (sharding, seeds, max-over-ranks timing, rank-0 gather)."""
+"""world_size-2 gloo test of the N>1 path's host logic (sharding, seeds, max-over-ranks timing, rank-0 gather, with and
+without the names)."""
 import os
 import socket
 
@@ -25,15 +26,16 @@ def _worker(rank, world, port, out):
         x = torch.randn(8, 4, 4, 12, generator=g)            # this rank's "sequence"
         ms = D.max_over_ranks(10.0 + 5.0 * rank, torch.device("cpu"))
         gathered = D.gather_on_rank0(x)
+        named = D.gather_named_on_rank0(x, [f"rank{rank}"])
         idx = D.shard_indices(5, rank, world)
         if rank == 0:
-            ok = len(gathered) == world
+            ok = len(gathered) == world and len(named) == world
             for r in range(world):
                 ref = torch.randn(8, 4, 4, 12, generator=torch.Generator().manual_seed(D.rank_seed(r)))
-                ok = ok and torch.equal(gathered[r], ref)
+                ok = ok and torch.equal(gathered[r], ref) and torch.equal(named[r][0], ref) and named[r][1] == [f"rank{r}"]
             out.put((rank, ok, ms, idx))
         else:
-            out.put((rank, gathered is None, ms, idx))
+            out.put((rank, gathered is None and named == [], ms, idx))
     finally:
         dist.destroy_process_group()
 
